@@ -1,6 +1,6 @@
-"""agogo_b200 — B200-native AlphaZero self-play engine behind gorgonia/agogo's API.
+"""agogo_b200 — H100-native AlphaZero self-play engine behind gorgonia/agogo's API.
 
-The compute lives in agogo_b200/libagogo_b200.so (hand-written sm_100a CUDA behind the C ABI of
+The compute lives in agogo_b200/libagogo_b200.so (hand-written sm_90a CUDA behind the C ABI of
 include/agogo_b200.h).  There is no CPU fallback: loading the engine without the built library,
 or creating an engine without a CUDA device, raises.
 """

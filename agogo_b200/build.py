@@ -1,4 +1,4 @@
-"""Builds agogo_b200/libagogo_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds agogo_b200/libagogo_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libagogo_b200.so")
 OBJ = os.path.join(HERE, "build")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
 # (file, extra flags).  -fmad=false: bit-exact PUCT / oracle-order fp32 arithmetic.
 UNITS = [

@@ -17,7 +17,7 @@ enum {
   ERR_NO_ACTIVE_CHILD = 1,   // node.go:232-234 panic("Cannot return nil")
   ERR_POOL_EXHAUSTED = 2,    // node pool of a tree is full
   ERR_ROOT_NO_CHILDREN = 4,  // search.go:141-149 fallback path (not implemented on device)
-  ERR_ACT_OVERFLOW = 8,      // tcgen05 tower: fp16 activation overflow (raise act_scale headroom)
+  ERR_ACT_OVERFLOW = 8,      // tensor-core tower: fp16 activation overflow (raise act_scale headroom)
   ERR_NAN_PRIOR = 16,        // NaN prior reached the sort (Go's sort order is unspecified there)
   ERR_PATH_OVERFLOW = 32,
   ERR_RESIGN_APPLIED = 64,   // Arena applies Resign: every game.State.Apply indexes board[-2] and panics

@@ -56,8 +56,6 @@ struct az_engine {
   EngineDev E;  // device pointers
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaStream_t stream2 = nullptr;                   // agent B's evaluation when both small-net towers fit the GPU side by side
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   std::vector<void*> allocs;
   std::vector<unsigned long long> zt64;  // host copy of the position keys (external states are hashed on the host)
   NetLayout L;
@@ -106,7 +104,7 @@ struct az_engine {
   int** d_peer_flags = nullptr;
   int* my_flags = nullptr;
   unsigned int* done_counter = nullptr;
-  int epoch = 0, num_sms = 148;
+  int epoch = 0, num_sms = 132;
   int32_t* d_agree = nullptr;  // step-count agreement of the data-parallel ranks (az_train)
   // Agent.Search on external positions: the position each agent's tree (game slot 0) was last searched on = t.prev
   struct ExtPrev { bool valid = false; int move_number = 0; std::vector<uint8_t> board; } ext_prev[2];
@@ -174,7 +172,7 @@ static int device_error_to_rc(az_engine* e, int bits) {
   if (bits & ERR_NO_ACTIVE_CHILD) m += " Cannot return nil (node.go:232: no selectable child)";
   if (bits & ERR_POOL_EXHAUSTED) m += " node pool exhausted (raise max_nodes_per_tree)";
   if (bits & ERR_ROOT_NO_CHILDREN) m += " root without children (search.go:141-149 fallback not implemented)";
-  if (bits & ERR_ACT_OVERFLOW) m += " fp16 activation overflow in the tcgen05 tower (lower act_scale_log2)";
+  if (bits & ERR_ACT_OVERFLOW) m += " fp16 activation overflow in the tensor-core tower (lower act_scale_log2)";
   if (bits & ERR_NAN_PRIOR) m += " NaN prior";
   if (bits & ERR_PATH_OVERFLOW) m += " per-game move capacity exceeded (set game.max_moves)";
   if (bits & ERR_RESIGN_APPLIED) m += " index out of range (Arena applied Resign: State.Apply indexes board[-2])";
@@ -185,7 +183,7 @@ static int device_error_to_rc(az_engine* e, int bits) {
 
 extern "C" {
 
-const char* az_build_info(void) { return "agogo_b200 0.1 sm_100a (hand-written CUDA; tcgen05/TMA tower; no CPU fallback)"; }
+const char* az_build_info(void) { return "agogo_b200 0.1 sm_90a (hand-written CUDA; wgmma/TMA tower; no CPU fallback)"; }
 const char* az_last_error(const az_engine* e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
 void az_engine_destroy(az_engine* e) {
@@ -215,9 +213,6 @@ void az_engine_destroy(az_engine* e) {
   if (e->h_ex_value) cudaFreeHost(e->h_ex_value);
   if (e->h_ex_valid) cudaFreeHost(e->h_ex_valid);
   if (e->h_small) cudaFreeHost(e->h_small);
-  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-  if (e->ev_join) cudaEventDestroy(e->ev_join);
-  if (e->stream2) cudaStreamDestroy(e->stream2);
   if (e->stream) cudaStreamDestroy(e->stream);
   delete e;
 }
@@ -253,9 +248,6 @@ int az_engine_create(const az_engine_desc* desc, az_engine** out) {
     e->device = desc->device;
     CUDA_CHECK(cudaSetDevice(e->device));
     CUDA_CHECK(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-    CUDA_CHECK(cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
-    CUDA_CHECK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    CUDA_CHECK(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
     GameP& P = e->P;
     P.kind = gd.kind; P.m = gd.m; P.n = gd.n; P.k = gd.k; P.cells = gd.m * gd.n;
     P.A = gd.kind == AZ_GAME_C4 ? gd.n : P.cells;
@@ -553,21 +545,8 @@ int az_arena_begin(az_engine* e, int32_t n_games, int32_t record) {
 
 static void eval_pending(az_engine* e) {
   launch_infer_simple(e->P, e->E, e->n_play, e->stream); e->launches++;
-  // the whole-net kernel of a small tower keeps one sample pair per CTA: two agents' batches fit the SMs side by side
-  // (fork / join through events: also what the captured wave graph records); the fused head scratch is per tower
-  const bool side_by_side = !e->P.shared_tree && e->use_tc && e->E.inf[0].kind == INF_DUAL && e->E.inf[1].kind == INF_DUAL &&
-                            tc_tower_kernel_kind(e->tc[0]) == 5;
-  if (side_by_side) {
-    CUDA_CHECK(cudaEventRecord(e->ev_fork, e->stream));
-    CUDA_CHECK(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
-    run_forward(e, 0);
-    run_forward(e, 1, e->stream2);
-    CUDA_CHECK(cudaEventRecord(e->ev_join, e->stream2));
-    CUDA_CHECK(cudaStreamWaitEvent(e->stream, e->ev_join, 0));
-  } else {
-    run_forward(e, 0);
-    if (!e->P.shared_tree) run_forward(e, 1);
-  }
+  run_forward(e, 0);
+  if (!e->P.shared_tree) run_forward(e, 1);
   launch_expand_backup(e->P, e->E, e->n_play, e->stream); e->launches++;
 }
 

@@ -1,7 +1,12 @@
-// agogo_b200 — shared pieces of the tcgen05 kernels (tower_tc.cu: inference tower, train_tc.cu: training GEMMs):
-// PTX wrappers (mbarrier, TMA, tcgen05), shared-memory / instruction descriptors, the single-CTA implicit-GEMM 3x3
-// convolution kernel template and the host-side tensor-map builders.  Everything lives in an anonymous namespace: each
-// translation unit instantiates what it launches.
+// agogo_b200 — shared pieces of the tensor-core kernels (tower_tc.cu: inference tower, train_tc.cu: training GEMMs):
+// PTX wrappers (mbarrier, TMA, wgmma), shared-memory matrix descriptors, the implicit-GEMM 3x3 convolution kernel
+// template and the host-side tensor-map builders.  Everything lives in an anonymous namespace: each translation unit
+// instantiates what it launches.
+//
+// Hopper (sm_90a) structure of every GEMM kernel here: warp 8 (lane 0) is the TMA producer filling a ring of K-block
+// stages (full/empty mbarriers); warps 0-7 are two consumer warpgroups, each owning 64 of the tile's 128 M rows and
+// issuing wgmma.mma_async (m64 x BN x k16, both operands from shared memory, fp32 accumulators in registers), then
+// running the epilogue straight from its registers while the producer already fills the next tile's stages.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -17,16 +22,16 @@
 namespace {
 
 
-constexpr int BM = 128;        // M tile (TMEM lanes)
-// K block per pipeline stage: 64 fp16 = 128 B rows (SWIZZLE_128B) or 32 fp16 = 64 B rows (SWIZZLE_64B, twice the
-// stages in the same shared memory).  Template parameter BKT of the kernel; chosen at tower allocation.
-constexpr int NTHREADS = 192;  // 6 warps
-__host__ __device__ constexpr int stage_bytes(int BN, int BKT) { return 2 * BM * BKT * 2 + 2 * BN * BKT * 2; }
-__host__ __device__ constexpr int num_stages(int BN, int BKT) { return 196608 / stage_bytes(BN, BKT) > 8 ? 8 : 196608 / stage_bytes(BN, BKT); }
-constexpr int AFF_BYTES = 4 * 2 * 4096;  // fused-pair epilogue: per epilogue warp two 32-row x 128-byte affine boxes (TMA, SWIZZLE_128B)
-__host__ __device__ constexpr int smem_bytes(int BN, int BKT, bool pair = false) {
-  return num_stages(BN, BKT) * stage_bytes(BN, BKT) + (pair ? AFF_BYTES : 0) + 1024 + 256;
-}
+constexpr int BM = 128;        // M tile: two consumer warpgroups x 64 rows
+constexpr int BK = 64;         // K block per pipeline stage: 64 fp16 = 128-byte rows (SWIZZLE_128B)
+constexpr int NTHREADS = 288;  // warps 0-7: two consumer warpgroups; warp 8: TMA producer
+constexpr int PRODUCER_WARP = 8;
+constexpr int CONSUMER_WARPS = 8;
+// H100: 227 KB of dynamic shared memory per block, less alignment slack and the barriers
+constexpr int SMEM_RING_BUDGET = 227 * 1024 - 2048;
+__host__ __device__ constexpr int stage_bytes(int BN) { return 2 * BM * BK * 2 + 2 * BN * BK * 2; }
+__host__ __device__ constexpr int num_stages(int BN) { return SMEM_RING_BUDGET / stage_bytes(BN) > 8 ? 8 : SMEM_RING_BUDGET / stage_bytes(BN); }
+__host__ __device__ constexpr int smem_bytes(int BN) { return num_stages(BN) * stage_bytes(BN) + 1024 + 256; }
 
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
@@ -64,59 +69,121 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads/writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16 inputs, fp32 accumulate), cta_group::1
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+
+// D (+)= A[smem] * B[smem], m64 x N x k16, fp16 inputs, fp32 accumulate; TB = 1: B is MN-major (transposed)
+template <int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 0, %35;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TB));
 }
-// K-major swizzled operand descriptor: start>>4 | LBO (ignored for swizzled K-major) | SBO = 8 rows x row bytes
-// (1024 B for SWIZZLE_128B, 512 B for SWIZZLE_64B) | version 1 (bits 46-47) | layout type (bits 61-63: 2 = 128B, 4 = 64B)
-template <int BKT>
+template <int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 0, %67;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, %131;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TB));
+}
+template <int N, int TB>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  if constexpr (N == 256) wgmma_n256<TB>(d, desc_a, desc_b, accumulate);
+  else if constexpr (N == 128) wgmma_n128<TB>(d, desc_a, desc_b, accumulate);
+  else wgmma_n64<TB>(d, desc_a, desc_b, accumulate);
+}
+
+// wgmma shared-memory matrix descriptor: start >> 4 (bits 0-13) | LBO >> 4 (16-29) | SBO >> 4 (32-45) |
+// layout type (bits 62-63: 1 = SWIZZLE_128B).  Tile bases are 1024-byte aligned, so the base offset (49-51) is 0.
+// K-major, SWIZZLE_128B: rows of 64 fp16, 8-row atoms 1024 B apart (SBO); LBO unused.
 __device__ __forceinline__ uint64_t make_desc_sw(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((8 * BKT * 2) >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(BKT == 64 ? 2 : 4) << 61;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// MN-major operand, SWIZZLE_128B: 64-element (128 B) runs along M/N, rows = K index; atoms of 8 K-rows (1024 B, SBO),
+// K-major, no swizzle: 8x16-byte core matrices, rows 16 B apart (8-row groups SBO = 128 B), 8-element K chunks lbo_bytes
+// apart (canonical layout ((8,m),(T,2k)):((1T,SBO),(1,LBO)) in 16-byte units).  Any 16-byte-aligned start is valid, so a
+// start `shift` rows into a tile is the same tile shifted by `shift` rows.
+__device__ __forceinline__ uint64_t make_desc_plain(uint32_t smem_addr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)(lbo_bytes >> 4) << 16;
+  d |= (uint64_t)(128 >> 4) << 32;
+  return d;
+}
+// MN-major, SWIZZLE_128B: 64-element (128 B) runs along M/N, rows = K index; atoms of 8 K-rows (1024 B, SBO),
 // 64-wide M/N groups lbo_bytes apart (canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units)
 __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)(lbo_bytes >> 4) << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// instruction descriptor: D=F32 (bits 4-5 = 1), A=B=F16 (0), K-major both, N>>3 at bit 17, M>>4 at bit 24
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // training operands carry a data-dependent power-of-two scale: the device word is ilogb(absmax) - 13 (or the
 // 0x80808080 fill when the tensor is all zero); scale exponent e = -word
@@ -143,46 +210,46 @@ struct ConvArgs {
   const int* exp_b;
 };
 
-template <int BN, bool PAIR, int BKT>
+// One K block of the three-pass product for this warpgroup's 64 rows: A rows at a_hi / a_lo, B (BN rows) at b_hi / b_lo.
+// a_step / b_step: descriptor start-address advance (16-byte units) per 16-wide K step.
+template <int BN, int TB>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t dAh, uint64_t dAl, uint64_t dBh, uint64_t dBl,
+                                           uint32_t b_step, bool first, int passes, uint32_t a_step = 32 >> 4) {
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < BK / 16; ks++) {
+    const uint64_t adv = (uint64_t)ks * a_step;     // A: K-major SWIZZLE_128B: 16 fp16 = 32 B inside the atom
+    const uint64_t advb = (uint64_t)ks * b_step;    // B: K-major as A; MN-major 16 K-rows of 128 B
+    wgmma_f16<BN, TB>(acc, dAh + adv, dBh + advb, (first && ks == 0) ? 0u : 1u);
+    if (passes >= 2) wgmma_f16<BN, TB>(acc, dAh + adv, dBl + advb, 1u);
+    if (passes >= 3) wgmma_f16<BN, TB>(acc, dAl + adv, dBh + advb, 1u);
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  acc_fence(acc);
+}
+
+template <int BN, bool PAIR>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-             const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-             const __grid_constant__ CUtensorMap tmAff, ConvArgs a) {
-  constexpr int BK = BKT;
+             const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, ConvArgs a) {
   constexpr int A_TILE_BYTES = BM * BK * 2;
-  constexpr int STAGES = num_stages(BN, BKT);
-  constexpr int STAGE_BYTES = stage_bytes(BN, BKT);
+  constexpr int STAGES = num_stages(BN);
+  constexpr int STAGE_BYTES = stage_bytes(BN);
   constexpr int B_TILE_BYTES = BN * BK * 2;
   constexpr int OUTC = PAIR ? BN / 2 : BN;  // output channels per N tile
-  constexpr int TMEM_COLS = 2 * BN >= 512 ? 512 : (2 * BN >= 256 ? 256 : 128);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  constexpr int AFF = PAIR ? AFF_BYTES : 0;
-  const uint32_t aff_smem = smem_base + STAGES * STAGE_BYTES;  // PAIR: 4 warps x 2 x 4 KB affine boxes (1024-aligned)
-  const uint32_t bars = aff_smem + AFF;  // full[S], empty[S], tfull[2], tempty[2], afull[4][2]
-  uint32_t* tmem_ptr_smem = (uint32_t*)(smem_al + STAGES * STAGE_BYTES + AFF + 240);
+  const uint32_t bars = smem_base + STAGES * STAGE_BYTES;  // full[S], empty[S]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int i) { return bars + 8u * (2 * STAGES + i); };
-  auto tempty_bar = [&](int i) { return bars + 8u * (2 * STAGES + 2 + i); };
-  auto afull_bar = [&](int quad, int buf) { return bars + 8u * (2 * STAGES + 4 + quad * 2 + buf); };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(tfull_bar(i), 1); mbar_init(tempty_bar(i), 4); }
-    for (int i = 0; i < 8; i++) mbar_init(afull_bar(i >> 1, i & 1), 1);
+    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int n = min(*a.n_dev, a.n_max);
   const int rows = n * a.S;
@@ -192,7 +259,7 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
   const int kc_per_tap = a.cin / BK;
   const int kblocks = 9 * kc_per_tap;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       // ===== TMA producer =====
       uint32_t it = 0;
@@ -221,166 +288,84 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer (single thread) =====
-      constexpr uint32_t idesc = make_idesc(BM, BN);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tcount++) {
-        const int acc = tcount & 1;
-        const uint32_t aph = (tcount >> 1) & 1;
-        mbar_wait(tempty_bar(acc), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kblocks; kb++, it++) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * STAGE_BYTES;
-          const uint64_t dAh = make_desc_sw<BKT>(sa), dAl = make_desc_sw<BKT>(sa + A_TILE_BYTES);
-          const uint64_t dBh = make_desc_sw<BKT>(sa + 2 * A_TILE_BYTES), dBl = make_desc_sw<BKT>(sa + 2 * A_TILE_BYTES + B_TILE_BYTES);
-#pragma unroll
-          for (int ks = 0; ks < BK / 16; ks++) {
-            const uint64_t adv = (uint64_t)(ks * 32 >> 4);  // 16 fp16 = 32 B along K inside the swizzle atom
-            umma_f16(d_tmem, dAh + adv, dBh + adv, idesc, (kb | ks) ? 1u : 0u);
-            if (a.passes >= 2) umma_f16(d_tmem, dAh + adv, dBl + adv, idesc, 1u);
-            if (a.passes >= 3) umma_f16(d_tmem, dAl + adv, dBh + adv, idesc, 1u);
-          }
-          umma_commit(empty_bar(s));  // frees the smem stage when the MMAs above have read it
-        }
-        umma_commit(tfull_bar(acc));  // accumulator complete
-      }
+    return;
+  }
+  // ===== consumer warpgroups 0 and 1: rows wg*64 .. wg*64+63 of the tile =====
+  const int wg = warp >> 2;
+  // accumulator fragment of m64nBNk16: acc[4j + 2h + e] = (row 16*(warp&3) + lane/4 + 8h, column 8j + 2*(lane&3) + e)
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+  float acc[BN / 2];
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
+    const int m0 = mt * BM, n0 = nt * BN;
+    for (int kb = 0; kb < kblocks; kb++, it++) {
+      const int s = it % STAGES;
+      const uint32_t ph = (it / STAGES) & 1;
+      mbar_wait(full_bar(s), ph);
+      __syncwarp();
+      const uint32_t sa = smem_base + s * STAGE_BYTES;
+      mma_kblock<BN, 0>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
+                        make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
+                        kb == 0, a.passes);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s));  // this warp's share of the stage has been read
     }
-  } else {
-    // ===== epilogue warps 2..5: TMEM lane quadrant = warp % 4 =====
-    const int quad = warp & 3;
-    uint32_t tcount = 0;
-    // Fused-pair layers: the per-(channel, point) affine of both branches ({A'a, Ba, A'b, Bb} per channel, rows = board
-    // positions in layout order) is staged through shared memory by TMA, 8 channels (= one 128-byte row) x this warp's
-    // 32 rows per box, double buffered and prefetched two boxes ahead across tiles.  (Reading it with per-thread global
-    // loads touches 32 cache lines per warp instruction: lane = row, 4 KB row pitch.)
-    constexpr int CH = OUTC / 8;  // boxes per tile
-    const uint32_t aff_buf = aff_smem + quad * 8192;
-    auto aff_issue = [&](uint32_t qq) {
-      if (!PAIR) return;
-      const int tile = blockIdx.x + (int)(qq / CH) * gridDim.x;
-      if (tile >= total_tiles) return;
-      const int j = qq % CH;
-      const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-      const int prow = a.mode3d ? (mt % a.tps) * BM + quad * 32 : (mt * BM + quad * 32) % a.S;
-      if (lane == 0) {
-        const uint32_t bar = afull_bar(quad, qq & 1);
-        mbar_expect_tx(bar, 4096);
-        tma_load_2d(aff_buf + (qq & 1) * 4096, &tmAff, bar, (nt * OUTC + j * 8) * 4, prow);
-      }
-    };
-    aff_issue(0);
-    aff_issue(1);
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, tcount++) {
-      const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-      const int m0 = mt * BM, n0 = nt * BN;
-      const int acc = tcount & 1;
-      const uint32_t aph = (tcount >> 1) & 1;
-      mbar_wait(tfull_bar(acc), aph);
-      tc_fence_after();
+    // ===== epilogue from registers =====
+    bool overflow = false;
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int lr = row0 + 8 * h;
       int r, p;  // r = row in the activation buffer (without guard), p = position inside the sample
       bool inb;
       if (a.mode3d) {
         const int b = mt / a.tps;
-        p = (mt - b * a.tps) * BM + quad * 32 + lane;
+        p = (mt - b * a.tps) * BM + lr;
         r = b * a.S + p;
         inb = p < a.S;
       } else {
-        r = m0 + quad * 32 + lane;
+        r = m0 + lr;
         p = r % a.S;
         inb = r < rows;
       }
       const int y = p / a.Wp, x = p - y * a.Wp;
       const bool valid = inb && y < a.H && x < a.W;
-      const int hw = y * a.W + x;
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN;
-      const float2* aff = a.aff + (size_t)(valid ? hw : 0) * a.n_total + n0;
-      __half* ohi = a.out_hi + (size_t)(a.guard + r) * a.cout + nt * OUTC;
-      __half* olo = a.out_lo + (size_t)(a.guard + r) * a.cout + nt * OUTC;
-      bool overflow = false;
-#pragma unroll 1
-      for (int c0 = 0; c0 < OUTC; c0 += 32) {
-        uint32_t ra[32], rb[32];
-        tmem_ld32(t_row + c0, ra);
-        if (PAIR) tmem_ld32(t_row + BN / 2 + c0, rb);
-        tmem_ld_wait();
-        if (a.out_raw) {
-          if (valid) {
-            const float sc = exp2f(-(float)(exp_decode(a.exp_a) + exp_decode(a.exp_b)));
-            float4* o = reinterpret_cast<float4*>(a.out_raw + (size_t)(a.guard + r) * a.n_total + n0 + c0);
+      if (!valid) continue;
+      if (a.out_raw) {
+        const float sc = exp2f(-(float)(exp_decode(a.exp_a) + exp_decode(a.exp_b)));
+        float* o = a.out_raw + (size_t)(a.guard + r) * a.n_total + n0 + col0;
 #pragma unroll
-            for (int q = 0; q < 8; q++)
-              o[q] = make_float4(__uint_as_float(ra[4 * q]) * sc, __uint_as_float(ra[4 * q + 1]) * sc,
-                                 __uint_as_float(ra[4 * q + 2]) * sc, __uint_as_float(ra[4 * q + 3]) * sc);
-          }
-        } else if (PAIR) {
-#pragma unroll
-          for (int sub = 0; sub < 4; sub++) {
-            const uint32_t qq = tcount * CH + (c0 >> 3) + sub;
-            mbar_wait(afull_bar(quad, qq & 1), (qq >> 1) & 1);
-            const uint8_t* box = smem_al + (aff_buf - smem_base) + (qq & 1) * 4096 + lane * 128;
-            __align__(16) __half hi[8];
-            __align__(16) __half lo[8];
-#pragma unroll
-            for (int k = 0; k < 8; k++) {
-              const float4 f = *reinterpret_cast<const float4*>(box + ((k ^ (lane & 7)) << 4));  // SWIZZLE_128B
-              const int i = sub * 8 + k;
-              float v = fmaxf(fmaf(f.x, __uint_as_float(ra[i]), f.y), 0.0f) + fmaxf(fmaf(f.z, __uint_as_float(rb[i]), f.w), 0.0f);
-              v *= a.act_scale;
-              const __half h = __float2half_rn(v);
-              const float hf = __half2float(h);
-              overflow |= valid && !(fabsf(hf) <= 65504.0f);
-              hi[k] = h;
-              lo[k] = __float2half_rn(v - hf);
-            }
-            if (valid) {
-              *(uint4*)(ohi + c0 + sub * 8) = *(const uint4*)hi;
-              *(uint4*)(olo + c0 + sub * 8) = *(const uint4*)lo;
-            }
-            __syncwarp();
-            aff_issue(qq + 2);
-          }
-        } else if (valid) {
-          __align__(16) __half hi[32];
-          __align__(16) __half lo[32];
-#pragma unroll
-          for (int i = 0; i < 32; i++) {
-            float2 fa = __ldg(aff + c0 + i);
-            float v = fmaxf(fmaf(fa.x, __uint_as_float(ra[i]), fa.y), 0.0f);
-            if (PAIR) {
-              float2 fb = __ldg(aff + BN / 2 + c0 + i);
-              v += fmaxf(fmaf(fb.x, __uint_as_float(rb[i]), fb.y), 0.0f);
-            }
-            v *= a.act_scale;
-            __half h = __float2half_rn(v);
-            float hf = __half2float(h);
-            overflow |= !(fabsf(hf) <= 65504.0f);
-            hi[i] = h;
-            lo[i] = __float2half_rn(v - hf);
-          }
-#pragma unroll
-          for (int q = 0; q < 4; q++) {
-            *(uint4*)(ohi + c0 + q * 8) = *(const uint4*)(hi + q * 8);
-            *(uint4*)(olo + c0 + q * 8) = *(const uint4*)(lo + q * 8);
-          }
-        }
+        for (int j = 0; j < BN / 8; j++)
+          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[4 * j + 2 * h] * sc, acc[4 * j + 2 * h + 1] * sc);
+        continue;
       }
-      if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
+      const int hw = y * a.W + x;
+      const float2* aff = a.aff + (size_t)hw * a.n_total + n0 + col0;
+      __half* ohi = a.out_hi + (size_t)(a.guard + r) * a.cout + nt * OUTC + col0;
+      __half* olo = a.out_lo + (size_t)(a.guard + r) * a.cout + nt * OUTC + col0;
+#pragma unroll
+      for (int j = 0; j < OUTC / 8; j++) {
+        __half hv[2], lv[2];
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const float2 fa = __ldg(aff + 8 * j + e);
+          float v = fmaxf(fmaf(fa.x, acc[4 * j + 2 * h + e], fa.y), 0.0f);
+          if (PAIR) {
+            const float2 fb = __ldg(aff + BN / 2 + 8 * j + e);
+            v += fmaxf(fmaf(fb.x, acc[4 * (j + OUTC / 8) + 2 * h + e], fb.y), 0.0f);
+          }
+          v *= a.act_scale;
+          const __half hh = __float2half_rn(v);
+          const float hf = __half2float(hh);
+          overflow |= !(fabsf(hf) <= 65504.0f);
+          hv[e] = hh;
+          lv[e] = __float2half_rn(v - hf);
+        }
+        *reinterpret_cast<__half2*>(ohi + 8 * j) = __halves2half2(hv[0], hv[1]);
+        *reinterpret_cast<__half2*>(olo + 8 * j) = __halves2half2(lv[0], lv[1]);
+      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
+    if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
   }
 }
 
@@ -399,41 +384,28 @@ EncodeTiledFn get_encode() {
   }
   return fn;
 }
-// 2-D fp16 row-major [rows][cols] tensor, box {bk cols, box_rows}, swizzle = row bytes of the box
-CUtensorMap make_map(void* base, uint64_t rows, uint64_t cols, uint32_t box_rows, int bk) {
+// 2-D fp16 row-major [rows][cols] tensor, box {64 cols = 128 B, box_rows}, SWIZZLE_128B
+CUtensorMap make_map(void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
   CUtensorMap m;
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {cols * 2};
-  cuuint32_t box[2] = {(cuuint32_t)bk, box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)BK, box_rows};
   cuuint32_t es[2] = {1, 1};
   CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
   return m;
 }
 
-// fused-pair affine: fp32 [rows = board positions][cols = 4 floats per channel], box {32 floats = 128 B, 32 rows}
-CUtensorMap make_map_aff(void* base, uint64_t rows, uint64_t cols) {
-  CUtensorMap m;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 4};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(affine) failed: " + std::to_string((int)r));
-  return m;
-}
-
 // per-sample layout: 3-D fp16 tensor [n][S][cols], box {64 cols, BM positions, 1 sample}
-CUtensorMap make_map3d(void* base, uint64_t n, uint64_t S, uint64_t cols, int bk, uint32_t box_rows = BM) {
+CUtensorMap make_map3d(void* base, uint64_t n, uint64_t S, uint64_t cols) {
   CUtensorMap m;
   cuuint64_t dims[3] = {cols, S, n};
   cuuint64_t strides[2] = {cols * 2, S * cols * 2};
-  cuuint32_t box[3] = {(cuuint32_t)bk, box_rows, 1};
+  cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)BM, 1};
   cuuint32_t es[3] = {1, 1, 1};
   CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(3d) failed: " + std::to_string((int)r));
   return m;
 }

@@ -1,4 +1,4 @@
-// agogo_b200 — K5: the residual tower as tcgen05 / TMEM / TMA implicit GEMMs (sm_100a only).
+// agogo_b200 — K5: the residual tower as wgmma / TMA implicit GEMMs (sm_90a).
 //
 // One kernel launch per conv layer (the init 3x3 conv, then one launch per shared block computing
 // BOTH parallel branches as a single C->2C contraction, dualnet/dual.go:59-73):
@@ -13,1210 +13,15 @@
 //     3-D tensor map [sample][position][channel] whose out-of-range positions are zero-filled by
 //     TMA, M-tiles never straddle samples (19x19: 3 tiles = 384 rows per 361 points vs 400);
 //   * fp32 fidelity on fp16 tensor cores: x = hi + lo and w = hi + lo (both pre-scaled by powers of
-//     two), three tcgen05.mma passes per K-step (hi*hi + hi*lo + lo*hi) into one fp32 TMEM
+//     two), three wgmma passes per K-step (hi*hi + hi*lo + lo*hi) into one fp32 register
 //     accumulator; the dropped lo*lo term is ~2^-22 relative;
-//   * warp roles: warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-//     warps 2-5 = epilogue (tcgen05.ld -> BN-affine + ReLU + branch add -> fp16 hi/lo split ->
-//     global).  smem ring of K-blocks (full/empty mbarriers), double-buffered TMEM accumulator
-//     (tmem_full/tmem_empty mbarriers), persistent CTAs striding over (M-tile, N-tile).
-// Descriptor bit layouts follow the PTX ISA tcgen05 "shared memory descriptor" / "instruction
-// descriptor" tables (cross-checked against cute/arch/mma_sm100_desc.hpp in the image).
-#include <cuda_fp8.h>
-
+//   * warp roles (tc_common.cuh): one TMA producer warp, two consumer warpgroups of 64 rows each;
+//     smem ring of K-blocks (full/empty mbarriers), persistent CTAs striding over (M-tile, N-tile),
+//     epilogue (BN-affine + ReLU + branch add -> fp16 hi/lo split -> global) from the accumulators.
+// Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" table of wgmma.
 #include "tc_common.cuh"
 
 namespace {
-
-// -------------------------------------------------------------------------------------------------
-// CTA-pair version of the fused residual-block layer (cta_group::2): two CTAs of a cluster compute a 256 x 256 tile,
-// each owning 128 rows of A (its own M tile) and HALF of the B tile (rank 0: the 128 branch-a filter rows, rank 1:
-// the 128 branch-b rows); the pair's tensor cores read each B half once for both SMs.  Per SM and K-step that is
-// 4 KB (A) + 4 KB (B half) of shared-memory reads instead of 4 + 8, and 64 KB instead of 96 KB of TMA fill per
-// stage — the 1-CTA kernel is bound by exactly that shared-memory traffic (MMA operand reads ~91 B/clk + fill
-// ~60 B/clk against 128 B/clk; profiles/r01_summary.md).  3 stages of 64 KB.
-//   * both producers signal the LEADER's full barrier (count 2, tx = 2 x 64 KB); the leader's single MMA thread issues
-//     tcgen05.mma.cta_group::2 (M = 256) and commits with multicast to both CTAs' empty / tmem-full barriers;
-//   * each CTA's epilogue warps read their own TMEM lanes and arrive on the leader's tmem-empty barrier (count 8).
-constexpr int STAGES2 = 3;
-constexpr int STAGE2_BYTES = 4 * BM * 64 * 2;  // A hi/lo (128 x 64) + B-half hi/lo (128 x 64) = 64 KB
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;    // clears the CTA-rank bit of a shared::cluster address -> the pair's even CTA
-__host__ __device__ constexpr int smem_bytes2() { return STAGES2 * STAGE2_BYTES + AFF_BYTES + 1024 + 256; }
-
-__device__ __forceinline__ void tma2_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx_cluster(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cluster.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma2_commit_mc(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma2_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-k_conv3x3_tc2(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-              const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
-              const __grid_constant__ CUtensorMap tmAff, ConvArgs a) {
-  constexpr int BK = 64, BN = 256, OUTC = 128;
-  constexpr int TILE_BYTES = BM * BK * 2;  // 16 KB: one 128 x 64 fp16 operand tile
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t aff_smem = smem_base + STAGES2 * STAGE2_BYTES;
-  const uint32_t bars = aff_smem + AFF_BYTES;  // full[3], empty[3], tfull[2], tempty[2], afull[4][2]
-  uint32_t* tmem_ptr_smem = (uint32_t*)(smem_al + STAGES2 * STAGE2_BYTES + AFF_BYTES + 240);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t rank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-  auto full_bar = [&](int s) { return bars + 8u * s; };
-  auto empty_bar = [&](int s) { return bars + 8u * (STAGES2 + s); };
-  auto tfull_bar = [&](int i) { return bars + 8u * (2 * STAGES2 + i); };
-  auto tempty_bar = [&](int i) { return bars + 8u * (2 * STAGES2 + 2 + i); };
-  auto afull_bar = [&](int quad, int buf) { return bars + 8u * (2 * STAGES2 + 4 + quad * 2 + buf); };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES2; s++) { mbar_init(full_bar(s), 2); mbar_init(empty_bar(s), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(tfull_bar(i), 1); mbar_init(tempty_bar(i), 8); }
-    for (int i = 0; i < 8; i++) mbar_init(afull_bar(i >> 1, i & 1), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // the peer's barriers are initialised before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  const int n = min(*a.n_dev, a.n_max);
-  const int rows = n * a.S;
-  const int m_tiles = a.mode3d ? n * a.tps : (rows + BM - 1) / BM;
-  const int m_pairs = (m_tiles + 1) / 2;
-  const int n_tiles = a.n_total / BN;
-  const int total_tiles = m_pairs * n_tiles;  // pair tiles (256 x 256)
-  const int kc_per_tap = a.cin / BK;
-  const int kblocks = 9 * kc_per_tap;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (both CTAs): own A tile + own half of B, all bytes counted on the leader's barrier =====
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters) {
-        const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-        const int mt = 2 * mp + (int)rank;
-        const int m0 = mt * BM, n0 = nt * BN + (int)rank * (BN / 2);
-        for (int kb = 0; kb < kblocks; kb++, it++) {
-          const int s = it % STAGES2;
-          const uint32_t ph = (it / STAGES2) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          const int tap = kb / kc_per_tap, kc = kb - tap * kc_per_tap;
-          const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-          const uint32_t sa = smem_base + s * STAGE2_BYTES;
-          const uint32_t lbar = full_bar(s) & PEER_MASK;
-          mbar_expect_tx_cluster(lbar, STAGE2_BYTES);
-          if (a.mode3d) {
-            const int b = mt / a.tps, p0 = (mt - b * a.tps) * BM + dy * a.Wp + dx;
-            tma2_load_3d(sa, &tmA_hi, lbar, kc * BK, p0, b);
-            tma2_load_3d(sa + TILE_BYTES, &tmA_lo, lbar, kc * BK, p0, b);
-          } else {
-            const int arow = a.guard + m0 + dy * a.Wp + dx;
-            tma2_load_2d(sa, &tmA_hi, lbar, kc * BK, arow);
-            tma2_load_2d(sa + TILE_BYTES, &tmA_lo, lbar, kc * BK, arow);
-          }
-          tma2_load_2d(sa + 2 * TILE_BYTES, &tmB_hi, lbar, tap * a.cin + kc * BK, n0);
-          tma2_load_2d(sa + 3 * TILE_BYTES, &tmB_lo, lbar, tap * a.cin + kc * BK, n0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ===== MMA issuer: the leader CTA's single thread drives both SMs =====
-      constexpr uint32_t idesc = make_idesc(2 * BM, BN);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, tcount++) {
-        const int acc = tcount & 1;
-        const uint32_t aph = (tcount >> 1) & 1;
-        mbar_wait(tempty_bar(acc), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kblocks; kb++, it++) {
-          const int s = it % STAGES2;
-          const uint32_t ph = (it / STAGES2) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * STAGE2_BYTES;
-          const uint64_t dAh = make_desc_sw<64>(sa), dAl = make_desc_sw<64>(sa + TILE_BYTES);
-          const uint64_t dBh = make_desc_sw<64>(sa + 2 * TILE_BYTES), dBl = make_desc_sw<64>(sa + 3 * TILE_BYTES);
-#pragma unroll
-          for (int ks = 0; ks < BK / 16; ks++) {
-            const uint64_t adv = (uint64_t)(ks * 32 >> 4);
-            umma2_f16(d_tmem, dAh + adv, dBh + adv, idesc, (kb | ks) ? 1u : 0u);
-            if (a.passes >= 2) umma2_f16(d_tmem, dAh + adv, dBl + adv, idesc, 1u);
-            if (a.passes >= 3) umma2_f16(d_tmem, dAl + adv, dBh + adv, idesc, 1u);
-          }
-          umma2_commit_mc(empty_bar(s));  // frees the stage in both CTAs
-        }
-        umma2_commit_mc(tfull_bar(acc));  // accumulators complete in both CTAs
-      }
-    }
-  } else {
-    // ===== epilogue warps 2..5 of either CTA: own 128 TMEM lanes =====
-    const int quad = warp & 3;
-    uint32_t tcount = 0;
-    constexpr int CH = OUTC / 8;
-    const uint32_t aff_buf = aff_smem + quad * 8192;
-    auto aff_issue = [&](uint32_t qq) {
-      const int tile = cluster_id + (int)(qq / CH) * n_clusters;
-      if (tile >= total_tiles) return;
-      const int j = qq % CH;
-      const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-      const int mt = 2 * mp + (int)rank;
-      const int prow = a.mode3d ? (mt % a.tps) * BM + quad * 32 : (mt * BM + quad * 32) % a.S;
-      if (lane == 0) {
-        const uint32_t bar = afull_bar(quad, qq & 1);
-        mbar_expect_tx(bar, 4096);
-        tma_load_2d(aff_buf + (qq & 1) * 4096, &tmAff, bar, (nt * OUTC + j * 8) * 4, prow);
-      }
-    };
-    aff_issue(0);
-    aff_issue(1);
-    for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, tcount++) {
-      const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-      const int mt = 2 * mp + (int)rank;
-      const int m0 = mt * BM;
-      const int acc = tcount & 1;
-      const uint32_t aph = (tcount >> 1) & 1;
-      mbar_wait(tfull_bar(acc), aph);
-      tc_fence_after();
-      int r, p;
-      bool inb;
-      if (a.mode3d) {
-        const int b = mt / a.tps;
-        p = (mt - b * a.tps) * BM + quad * 32 + lane;
-        r = b * a.S + p;
-        inb = p < a.S && mt < m_tiles;
-      } else {
-        r = m0 + quad * 32 + lane;
-        p = r % a.S;
-        inb = r < rows;
-      }
-      const int y = p / a.Wp, x = p - y * a.Wp;
-      const bool valid = inb && y < a.H && x < a.W;
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN;
-      __half* ohi = a.out_hi + (size_t)(a.guard + r) * a.cout + nt * OUTC;
-      __half* olo = a.out_lo + (size_t)(a.guard + r) * a.cout + nt * OUTC;
-      bool overflow = false;
-#pragma unroll 1
-      for (int c0 = 0; c0 < OUTC; c0 += 32) {
-        uint32_t ra[32], rb[32];
-        tmem_ld32(t_row + c0, ra);
-        tmem_ld32(t_row + BN / 2 + c0, rb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int sub = 0; sub < 4; sub++) {
-          const uint32_t qq = tcount * CH + (c0 >> 3) + sub;
-          mbar_wait(afull_bar(quad, qq & 1), (qq >> 1) & 1);
-          const uint8_t* box = smem_al + (aff_buf - smem_base) + (qq & 1) * 4096 + lane * 128;
-          __align__(16) __half hi[8];
-          __align__(16) __half lo[8];
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            const float4 f = *reinterpret_cast<const float4*>(box + ((k ^ (lane & 7)) << 4));
-            const int i = sub * 8 + k;
-            float v = fmaxf(fmaf(f.x, __uint_as_float(ra[i]), f.y), 0.0f) + fmaxf(fmaf(f.z, __uint_as_float(rb[i]), f.w), 0.0f);
-            v *= a.act_scale;
-            const __half h = __float2half_rn(v);
-            const float hf = __half2float(h);
-            overflow |= valid && !(fabsf(hf) <= 65504.0f);
-            hi[k] = h;
-            lo[k] = __float2half_rn(v - hf);
-          }
-          if (valid) {
-            *(uint4*)(ohi + c0 + sub * 8) = *(const uint4*)hi;
-            *(uint4*)(olo + c0 + sub * 8) = *(const uint4*)lo;
-          }
-          __syncwarp();
-          aff_issue(qq + 2);
-        }
-      }
-      if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(tempty_bar(acc) & PEER_MASK);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // nobody leaves while the peer may still signal its barriers / read its B half
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-  }
-}
-
-// -------------------------------------------------------------------------------------------------
-// Per-tap twin of the FP8-correction layer (AZ_TC_FP8=1: A/B against the halo kernel below, which is what AZ_FLAG_FAST_TOWER
-// runs; DESIGN.md §4 "Precision policy", tools/precision_study_fp8.py): the CTA-pair layer with
-// its two correction passes on the FP8 tensor path.  acc = hi16(x)·hi16(w)  [kind::f16]
-//                                                         + e4m3(hi·2^pa)·e4m3(w_lo·2^-pa) + e4m3(x_lo·2^q)·e4m3(w_hi·2^-q)  [kind::f8f6f4]
-// — every product carries the accumulator's scale, so the three kinds accumulate into the same fp32 TMEM tile.  FP8 MMAs
-// take K = 32 per instruction at twice the fp16 rate: 4 + 2 + 2 instructions per 64-wide K block instead of 12.
-// Activations travel as hi16 + lo16 (the heads and the next layer's re-split need lo16) + h8 + l8; a stage holds
-// A16 16 KB | A_h8 8 KB | A_l8 8 KB | B16 16 KB | B_h8 8 KB | B_l8 8 KB = 64 KB as before (fp8 tiles: 64-byte rows, SWIZZLE_64B).
-struct ConvArgsF8 {
-  ConvArgs c;
-  uint8_t* out_h8;  // [(guard + rows)][cout] e4m3(hi16 * 2^pa)
-  uint8_t* out_l8;  // [(guard + rows)][cout] e4m3(lo * 2^q)
-  float scale_h8, scale_l8;  // 2^pa, 2^q
-};
-__device__ __forceinline__ void umma2_f8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ uint8_t to_e5m2(float v) { return (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E5M2); }
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-k_conv3x3_tc2_f8(const __grid_constant__ CUtensorMap tmA16, const __grid_constant__ CUtensorMap tmAh8,
-                 const __grid_constant__ CUtensorMap tmAl8, const __grid_constant__ CUtensorMap tmB16,
-                 const __grid_constant__ CUtensorMap tmBh8, const __grid_constant__ CUtensorMap tmBl8,
-                 const __grid_constant__ CUtensorMap tmAff, ConvArgsF8 af) {
-  const ConvArgs& a = af.c;
-  constexpr int BK = 64, BN = 256, OUTC = 128;
-  constexpr int T16 = BM * BK * 2, T8 = BM * BK;  // 16 KB / 8 KB operand tiles (128 rows)
-  constexpr int OFF_AH8 = T16, OFF_AL8 = T16 + T8, OFF_B16 = T16 + 2 * T8, OFF_BH8 = 2 * T16 + 2 * T8, OFF_BL8 = 2 * T16 + 3 * T8;
-  static_assert(2 * T16 + 4 * T8 == STAGE2_BYTES, "stage layout");
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t aff_smem = smem_base + STAGES2 * STAGE2_BYTES;
-  const uint32_t bars = aff_smem + AFF_BYTES;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(smem_al + STAGES2 * STAGE2_BYTES + AFF_BYTES + 240);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t rank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-  auto full_bar = [&](int s) { return bars + 8u * s; };
-  auto empty_bar = [&](int s) { return bars + 8u * (STAGES2 + s); };
-  auto tfull_bar = [&](int i) { return bars + 8u * (2 * STAGES2 + i); };
-  auto tempty_bar = [&](int i) { return bars + 8u * (2 * STAGES2 + 2 + i); };
-  auto afull_bar = [&](int quad, int buf) { return bars + 8u * (2 * STAGES2 + 4 + quad * 2 + buf); };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES2; s++) { mbar_init(full_bar(s), 2); mbar_init(empty_bar(s), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(tfull_bar(i), 1); mbar_init(tempty_bar(i), 8); }
-    for (int i = 0; i < 8; i++) mbar_init(afull_bar(i >> 1, i & 1), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  const int n = min(*a.n_dev, a.n_max);
-  const int rows = n * a.S;
-  const int m_tiles = a.mode3d ? n * a.tps : (rows + BM - 1) / BM;
-  const int m_pairs = (m_tiles + 1) / 2;
-  const int n_tiles = a.n_total / BN;
-  const int total_tiles = m_pairs * n_tiles;
-  const int kc_per_tap = a.cin / BK;
-  const int kblocks = 9 * kc_per_tap;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters) {
-        const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-        const int mt = 2 * mp + (int)rank;
-        const int m0 = mt * BM, n0 = nt * BN + (int)rank * (BN / 2);
-        for (int kb = 0; kb < kblocks; kb++, it++) {
-          const int s = it % STAGES2;
-          const uint32_t ph = (it / STAGES2) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          const int tap = kb / kc_per_tap, kc = kb - tap * kc_per_tap;
-          const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-          const uint32_t sa = smem_base + s * STAGE2_BYTES;
-          const uint32_t lbar = full_bar(s) & PEER_MASK;
-          mbar_expect_tx_cluster(lbar, STAGE2_BYTES);
-          if (a.mode3d) {
-            const int b = mt / a.tps, p0 = (mt - b * a.tps) * BM + dy * a.Wp + dx;
-            tma2_load_3d(sa, &tmA16, lbar, kc * BK, p0, b);
-            tma2_load_3d(sa + OFF_AH8, &tmAh8, lbar, kc * BK, p0, b);
-            tma2_load_3d(sa + OFF_AL8, &tmAl8, lbar, kc * BK, p0, b);
-          } else {
-            const int arow = a.guard + m0 + dy * a.Wp + dx;
-            tma2_load_2d(sa, &tmA16, lbar, kc * BK, arow);
-            tma2_load_2d(sa + OFF_AH8, &tmAh8, lbar, kc * BK, arow);
-            tma2_load_2d(sa + OFF_AL8, &tmAl8, lbar, kc * BK, arow);
-          }
-          const int kcol = tap * a.cin + kc * BK;
-          tma2_load_2d(sa + OFF_B16, &tmB16, lbar, kcol, n0);
-          tma2_load_2d(sa + OFF_BH8, &tmBh8, lbar, kcol, n0);
-          tma2_load_2d(sa + OFF_BL8, &tmBl8, lbar, kcol, n0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      constexpr uint32_t idesc = make_idesc(2 * BM, BN);  // kind::f16: F16 x F16
-      constexpr uint32_t idesc8 = idesc | (1u << 7);      // kind::f8f6f4: A = E5M2 (activations), B = E4M3 (filters)
-      uint32_t it = 0, tcount = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, tcount++) {
-        const int acc = tcount & 1;
-        const uint32_t aph = (tcount >> 1) & 1;
-        mbar_wait(tempty_bar(acc), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < kblocks; kb++, it++) {
-          const int s = it % STAGES2;
-          const uint32_t ph = (it / STAGES2) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * STAGE2_BYTES;
-          const uint64_t dA16 = make_desc_sw<64>(sa), dB16 = make_desc_sw<64>(sa + OFF_B16);
-          // fp8 tiles: 64-byte rows = the SWIZZLE_64B form of the descriptor (what make_desc_sw<32> encodes for fp16)
-          const uint64_t dAh8 = make_desc_sw<32>(sa + OFF_AH8), dAl8 = make_desc_sw<32>(sa + OFF_AL8);
-          const uint64_t dBh8 = make_desc_sw<32>(sa + OFF_BH8), dBl8 = make_desc_sw<32>(sa + OFF_BL8);
-#pragma unroll
-          for (int ks = 0; ks < 4; ks++)  // 16 fp16 = 32 B per step
-            umma2_f16(d_tmem, dA16 + (uint64_t)(ks * 2), dB16 + (uint64_t)(ks * 2), idesc, (kb | ks) ? 1u : 0u);
-#pragma unroll
-          for (int ks = 0; ks < 2; ks++) {  // 32 fp8 = 32 B per step
-            umma2_f8(d_tmem, dAh8 + (uint64_t)(ks * 2), dBl8 + (uint64_t)(ks * 2), idesc8, 1u);
-            umma2_f8(d_tmem, dAl8 + (uint64_t)(ks * 2), dBh8 + (uint64_t)(ks * 2), idesc8, 1u);
-          }
-          umma2_commit_mc(empty_bar(s));
-        }
-        umma2_commit_mc(tfull_bar(acc));
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    uint32_t tcount = 0;
-    constexpr int CH = OUTC / 8;
-    const uint32_t aff_buf = aff_smem + quad * 8192;
-    auto aff_issue = [&](uint32_t qq) {
-      const int tile = cluster_id + (int)(qq / CH) * n_clusters;
-      if (tile >= total_tiles) return;
-      const int j = qq % CH;
-      const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-      const int mt = 2 * mp + (int)rank;
-      const int prow = a.mode3d ? (mt % a.tps) * BM + quad * 32 : (mt * BM + quad * 32) % a.S;
-      if (lane == 0) {
-        const uint32_t bar = afull_bar(quad, qq & 1);
-        mbar_expect_tx(bar, 4096);
-        tma_load_2d(aff_buf + (qq & 1) * 4096, &tmAff, bar, (nt * OUTC + j * 8) * 4, prow);
-      }
-    };
-    aff_issue(0);
-    aff_issue(1);
-    for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, tcount++) {
-      const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-      const int mt = 2 * mp + (int)rank;
-      const int m0 = mt * BM;
-      const int acc = tcount & 1;
-      const uint32_t aph = (tcount >> 1) & 1;
-      mbar_wait(tfull_bar(acc), aph);
-      tc_fence_after();
-      int r, p;
-      bool inb;
-      if (a.mode3d) {
-        const int b = mt / a.tps;
-        p = (mt - b * a.tps) * BM + quad * 32 + lane;
-        r = b * a.S + p;
-        inb = p < a.S && mt < m_tiles;
-      } else {
-        r = m0 + quad * 32 + lane;
-        p = r % a.S;
-        inb = r < rows;
-      }
-      const int y = p / a.Wp, x = p - y * a.Wp;
-      const bool valid = inb && y < a.H && x < a.W;
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN;
-      const size_t orow = (size_t)(a.guard + r) * a.cout + nt * OUTC;
-      bool overflow = false;
-#pragma unroll 1
-      for (int c0 = 0; c0 < OUTC; c0 += 32) {
-        uint32_t ra[32], rb[32];
-        tmem_ld32(t_row + c0, ra);
-        tmem_ld32(t_row + BN / 2 + c0, rb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int sub = 0; sub < 4; sub++) {
-          const uint32_t qq = tcount * CH + (c0 >> 3) + sub;
-          mbar_wait(afull_bar(quad, qq & 1), (qq >> 1) & 1);
-          const uint8_t* box = smem_al + (aff_buf - smem_base) + (qq & 1) * 4096 + lane * 128;
-          __align__(16) __half hi[8];
-          __align__(16) __half lo[8];
-          __align__(8) uint8_t h8[8];
-          __align__(8) uint8_t l8[8];
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            const float4 f = *reinterpret_cast<const float4*>(box + ((k ^ (lane & 7)) << 4));
-            const int i = sub * 8 + k;
-            float v = fmaxf(fmaf(f.x, __uint_as_float(ra[i]), f.y), 0.0f) + fmaxf(fmaf(f.z, __uint_as_float(rb[i]), f.w), 0.0f);
-            v *= a.act_scale;
-            const __half h = __float2half_rn(v);
-            const float hf = __half2float(h);
-            overflow |= valid && !(fabsf(hf) <= 65504.0f);
-            const float res = v - hf;
-            hi[k] = h;
-            lo[k] = __float2half_rn(res);
-            h8[k] = to_e5m2(hf * af.scale_h8);
-            l8[k] = to_e5m2(res * af.scale_l8);
-          }
-          if (valid) {
-            *(uint4*)(a.out_hi + orow + c0 + sub * 8) = *(const uint4*)hi;
-            *(uint4*)(a.out_lo + orow + c0 + sub * 8) = *(const uint4*)lo;
-            *(uint2*)(af.out_h8 + orow + c0 + sub * 8) = *(const uint2*)h8;
-            *(uint2*)(af.out_l8 + orow + c0 + sub * 8) = *(const uint2*)l8;
-          }
-          __syncwarp();
-          aff_issue(qq + 2);
-        }
-      }
-      if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(tempty_bar(acc) & PEER_MASK);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-  }
-}
-// -------------------------------------------------------------------------------------------------
-// Halo form of the FP8-correction layer (the product path of the fused layers, AZ_TC_FP8 unset or 2).
-// The per-tap kernel above re-loads the activation tile nine times per 64-channel chunk (one shifted 128-row box per
-// tap): 64 KB of shared-memory fill per K block on top of the 64 KB the tensor cores read — with the FP8 corrections a
-// K block is 8 MMA slots (1024 clk), so fill + operand reads need 128 B/clk, the whole shared-memory bandwidth of the SM
-// (ncu: tensor pipe 78 % active, profiles/r02_summary.md).  Here ONE box of BM + 2*(Wp+1) consecutive board positions
-// (170 -> 176 rows for 19x19) is loaded per (tile, 64-channel chunk) and the nine taps are row-shifted views of it: the
-// operand descriptor simply starts (Wp+1) + dy*Wp + dx rows into the tile.  TMA and the tensor core both apply the
-// 128B / 64B swizzle to absolute shared-memory address bits, so a start address that is row- but not pattern-aligned
-// reads what TMA wrote (base-offset field 0; tools/probe_rowshift.cu, profiles/r02_probe_rowshift.txt: exact for every
-// shift, fp16/SWIZZLE_128B and fp8/SWIZZLE_64B).  Loop order kc outer, tap inner; activation stages (2 x hrows x 256 B)
-// and filter stages (3 x 32 KB) have their own full/empty barriers.  Fill per K block: 32 KB of filters + 1/9 of a
-// 44 KB activation stage = 37 KB instead of 64 KB.
-// Activation correction operands are E5M2 at the fp16 operand's own scale — h8 = e5m2(hi16), l8 = e5m2(lo * 2^11) — so
-// they can neither saturate nor flush before fp16 itself does (E4M3's 2^-9..448 range did both on heavy-tailed
-// activations); filters stay E4M3 (static, scaled exactly per layer): w_l8 = e4m3(w_lo), w_h8 = e4m3(w_hi * 2^-11).
-constexpr int NBST = 3;
-constexpr int BST_BYTES = 2 * BM * 64 + 2 * BM * 64;  // B16 16 KB | B_h8 8 KB | B_l8 8 KB
-__host__ __device__ constexpr int smem_bytes_f8h(int hrows) { return 2 * hrows * 256 + NBST * BST_BYTES + AFF_BYTES + 1024 + 256; }
-constexpr int F8H_MAX_HROWS = 176;
-
-struct ConvArgsF8H {
-  ConvArgs c;
-  uint8_t* out_h8;  // [(guard + rows)][cout] e5m2(hi16)
-  uint8_t* out_l8;  // [(guard + rows)][cout] e5m2(lo * 2^11)
-  float scale_l8;   // 2^11
-  int hrows;        // rows of an activation stage: BM + 2*halo rounded up to 16
-  int halo;         // Wp + 1
-};
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-
-// F8 = true: hi*hi (kind::f16) + two FP8 correction passes.  F8 = false: the fp32-faithful three fp16 passes
-// (hi*hi + hi*lo + lo*hi) on the same halo pipeline — the stages then hold hi16 | lo16 of the activations
-// (tmAh8 = the lo16 halo map, tmAl8 unused) and hi16 | lo16 of the filters (tmBh8 = the lo16 map, tmBl8 unused).
-template <bool F8>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NTHREADS, 1)
-k_conv3x3_tc2_halo(const __grid_constant__ CUtensorMap tmA16, const __grid_constant__ CUtensorMap tmAh8,
-                   const __grid_constant__ CUtensorMap tmAl8, const __grid_constant__ CUtensorMap tmB16,
-                   const __grid_constant__ CUtensorMap tmBh8, const __grid_constant__ CUtensorMap tmBl8,
-                   const __grid_constant__ CUtensorMap tmAff, ConvArgsF8H af) {
-  const ConvArgs& a = af.c;
-  constexpr int BK = 64, BN = 256, OUTC = 128;
-  constexpr int T16 = BM * BK * 2, T8 = BM * BK;  // filter tiles: 16 KB / 8 KB (128 rows each)
-  const uint32_t A16_BYTES = (uint32_t)af.hrows * 128u, A8_BYTES = (uint32_t)af.hrows * 64u, AST_BYTES = (uint32_t)af.hrows * 256u;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t w_smem = smem_base + 2 * AST_BYTES;
-  const uint32_t aff_smem = w_smem + NBST * BST_BYTES;
-  const uint32_t bars = aff_smem + AFF_BYTES;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(smem_al + (bars - smem_base) + 240);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint32_t rank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-  auto xfull_bar = [&](int s) { return bars + 8u * s; };                   // activation stages
-  auto xempty_bar = [&](int s) { return bars + 8u * (2 + s); };
-  auto wfull_bar = [&](int s) { return bars + 8u * (4 + s); };             // filter stages
-  auto wempty_bar = [&](int s) { return bars + 8u * (4 + NBST + s); };
-  auto tfull_bar = [&](int i) { return bars + 8u * (4 + 2 * NBST + i); };
-  auto tempty_bar = [&](int i) { return bars + 8u * (6 + 2 * NBST + i); };
-  auto afull_bar = [&](int quad, int buf) { return bars + 8u * (8 + 2 * NBST + quad * 2 + buf); };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; s++) { mbar_init(xfull_bar(s), 2); mbar_init(xempty_bar(s), 1); }
-    for (int s = 0; s < NBST; s++) { mbar_init(wfull_bar(s), 2); mbar_init(wempty_bar(s), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(tfull_bar(i), 1); mbar_init(tempty_bar(i), 8); }
-    for (int i = 0; i < 8; i++) mbar_init(afull_bar(i >> 1, i & 1), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  const int n = min(*a.n_dev, a.n_max);
-  const int rows = n * a.S;
-  const int m_tiles = a.mode3d ? n * a.tps : (rows + BM - 1) / BM;
-  const int m_pairs = (m_tiles + 1) / 2;
-  const int n_tiles = a.n_total / BN;
-  const int total_tiles = m_pairs * n_tiles;
-  const int kcn = a.cin / BK;
-  const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-  const uint32_t my_tiles = cluster_id < total_tiles ? (uint32_t)((total_tiles - cluster_id + n_clusters - 1) / n_clusters) : 0u;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (both CTAs): own activation halo tile + own half of the filter tile =====
-      const uint32_t total_x = my_tiles * (uint32_t)kcn, total_w = total_x * 9u;
-      uint32_t xi = 0;
-      auto issue_x = [&](uint32_t i) {
-        const int tl = (int)(i / (uint32_t)kcn), kc = (int)i - tl * kcn;
-        const int tile = cluster_id + tl * n_clusters;
-        const int mt = 2 * (tile / n_tiles) + (int)rank;
-        const uint32_t sa = smem_base + (i & 1u) * AST_BYTES;
-        const uint32_t lbar = xfull_bar((int)(i & 1u)) & PEER_MASK;
-        mbar_expect_tx_cluster(lbar, AST_BYTES);
-        if (a.mode3d) {
-          const int b = mt / a.tps, p0 = (mt - b * a.tps) * BM - af.halo;  // <0 / >=S / b>=n: TMA zero fill
-          tma2_load_3d(sa, &tmA16, lbar, kc * BK, p0, b);
-          tma2_load_3d(sa + A16_BYTES, &tmAh8, lbar, kc * BK, p0, b);
-          if (F8) tma2_load_3d(sa + A16_BYTES + A8_BYTES, &tmAl8, lbar, kc * BK, p0, b);
-        } else {
-          const int arow = a.guard + mt * BM - af.halo;
-          tma2_load_2d(sa, &tmA16, lbar, kc * BK, arow);
-          tma2_load_2d(sa + A16_BYTES, &tmAh8, lbar, kc * BK, arow);
-          if (F8) tma2_load_2d(sa + A16_BYTES + A8_BYTES, &tmAl8, lbar, kc * BK, arow);
-        }
-      };
-      for (uint32_t t = 0; t < total_w; t++) {
-        const uint32_t i = t / 9u;
-        // activation stage i must be in flight before its filters; stage i+1 is prefetched as soon as its buffer is free
-        while (xi < total_x && xi <= i + 1u) {
-          const uint32_t par = ((xi >> 1) & 1u) ^ 1u;
-          if (xi <= i) mbar_wait(xempty_bar((int)(xi & 1u)), par);
-          else if (!mbar_test(xempty_bar((int)(xi & 1u)), par)) break;
-          issue_x(xi);
-          xi++;
-        }
-        const int tap = (int)(t - i * 9u);
-        const int tl = (int)(i / (uint32_t)kcn), kc = (int)i - tl * kcn;
-        const int tile = cluster_id + tl * n_clusters;
-        const int nt = tile % n_tiles;
-        const int n0 = nt * BN + (int)rank * (BN / 2);
-        const int s = (int)(t % NBST);
-        mbar_wait(wempty_bar(s), ((t / NBST) & 1u) ^ 1u);
-        const uint32_t sb = w_smem + s * BST_BYTES;
-        const uint32_t lbar = wfull_bar(s) & PEER_MASK;
-        mbar_expect_tx_cluster(lbar, BST_BYTES);
-        const int kcol = tap * a.cin + kc * BK;
-        tma2_load_2d(sb, &tmB16, lbar, kcol, n0);
-        tma2_load_2d(sb + T16, &tmBh8, lbar, kcol, n0);
-        if (F8) tma2_load_2d(sb + T16 + T8, &tmBl8, lbar, kcol, n0);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ===== MMA issuer: the leader CTA's single thread drives both SMs =====
-      constexpr uint32_t idesc16 = make_idesc(2 * BM, BN);
-      constexpr uint32_t idesc8 = idesc16 | (1u << 7);  // kind::f8f6f4: A = E5M2 (1), B = E4M3 (0)
-      uint32_t xi = 0, t = 0, tcount = 0;
-      for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, tcount++) {
-        const int acc = tcount & 1;
-        mbar_wait(tempty_bar(acc), ((tcount >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kc = 0; kc < kcn; kc++, xi++) {
-          mbar_wait(xfull_bar((int)(xi & 1u)), (xi >> 1) & 1u);
-          tc_fence_after();
-          const uint32_t sa = smem_base + (xi & 1u) * AST_BYTES;
-#pragma unroll 1
-          for (int tap = 0; tap < 9; tap++, t++) {
-            const int s = (int)(t % NBST);
-            mbar_wait(wfull_bar(s), (t / NBST) & 1u);
-            tc_fence_after();
-            const int dy = tap / 3 - 1, dx = tap - (tap / 3) * 3 - 1;
-            const uint32_t j0 = (uint32_t)(af.halo + dy * a.Wp + dx);  // first row of this tap's view of the halo tile
-            const uint32_t sb = w_smem + s * BST_BYTES;
-            const uint64_t dA16 = make_desc_sw<64>(sa + j0 * 128u);
-            const uint64_t dB16 = make_desc_sw<64>(sb);
-            if (F8) {
-              const uint64_t dAh8 = make_desc_sw<32>(sa + A16_BYTES + j0 * 64u);
-              const uint64_t dAl8 = make_desc_sw<32>(sa + A16_BYTES + A8_BYTES + j0 * 64u);
-              const uint64_t dBh8 = make_desc_sw<32>(sb + T16), dBl8 = make_desc_sw<32>(sb + T16 + T8);
-#pragma unroll
-              for (int ks = 0; ks < 4; ks++)  // 16 fp16 = 32 B per step
-                umma2_f16(d_tmem, dA16 + (uint64_t)(ks * 2), dB16 + (uint64_t)(ks * 2), idesc16, (kc | tap | ks) ? 1u : 0u);
-#pragma unroll
-              for (int ks = 0; ks < 2; ks++) {  // 32 fp8 = 32 B per step
-                umma2_f8(d_tmem, dAh8 + (uint64_t)(ks * 2), dBl8 + (uint64_t)(ks * 2), idesc8, 1u);
-                umma2_f8(d_tmem, dAl8 + (uint64_t)(ks * 2), dBh8 + (uint64_t)(ks * 2), idesc8, 1u);
-              }
-            } else {
-              const uint64_t dAlo = make_desc_sw<64>(sa + A16_BYTES + j0 * 128u), dBlo = make_desc_sw<64>(sb + T16);
-#pragma unroll
-              for (int ks = 0; ks < 4; ks++) {
-                const uint64_t adv = (uint64_t)(ks * 2);
-                umma2_f16(d_tmem, dA16 + adv, dB16 + adv, idesc16, (kc | tap | ks) ? 1u : 0u);
-                umma2_f16(d_tmem, dA16 + adv, dBlo + adv, idesc16, 1u);
-                umma2_f16(d_tmem, dAlo + adv, dB16 + adv, idesc16, 1u);
-              }
-            }
-            umma2_commit_mc(wempty_bar(s));
-          }
-          umma2_commit_mc(xempty_bar((int)(xi & 1u)));
-        }
-        umma2_commit_mc(tfull_bar(acc));
-      }
-    }
-  } else {
-    // ===== epilogue warps 2..5 of either CTA: own 128 TMEM lanes =====
-    const int quad = warp & 3;
-    uint32_t tcount = 0;
-    constexpr int CH = OUTC / 8;
-    const uint32_t aff_buf = aff_smem + quad * 8192;
-    auto aff_issue = [&](uint32_t qq) {
-      const int tile = cluster_id + (int)(qq / CH) * n_clusters;
-      if (tile >= total_tiles) return;
-      const int j = qq % CH;
-      const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-      const int mt = 2 * mp + (int)rank;
-      const int prow = a.mode3d ? (mt % a.tps) * BM + quad * 32 : (mt * BM + quad * 32) % a.S;
-      if (lane == 0) {
-        const uint32_t bar = afull_bar(quad, qq & 1);
-        mbar_expect_tx(bar, 4096);
-        tma_load_2d(aff_buf + (qq & 1) * 4096, &tmAff, bar, (nt * OUTC + j * 8) * 4, prow);
-      }
-    };
-    aff_issue(0);
-    aff_issue(1);
-    for (int tile = cluster_id; tile < total_tiles; tile += n_clusters, tcount++) {
-      const int mp = tile / n_tiles, nt = tile - mp * n_tiles;
-      const int mt = 2 * mp + (int)rank;
-      const int m0 = mt * BM;
-      const int acc = tcount & 1;
-      mbar_wait(tfull_bar(acc), (tcount >> 1) & 1u);
-      tc_fence_after();
-      int r, p;
-      bool inb;
-      if (a.mode3d) {
-        const int b = mt / a.tps;
-        p = (mt - b * a.tps) * BM + quad * 32 + lane;
-        r = b * a.S + p;
-        inb = p < a.S && mt < m_tiles;
-      } else {
-        r = m0 + quad * 32 + lane;
-        p = r % a.S;
-        inb = r < rows;
-      }
-      const int y = p / a.Wp, x = p - y * a.Wp;
-      const bool valid = inb && y < a.H && x < a.W;
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN;
-      const size_t orow = (size_t)(a.guard + r) * a.cout + nt * OUTC;
-      bool overflow = false;
-#pragma unroll 1
-      for (int c0 = 0; c0 < OUTC; c0 += 32) {
-        uint32_t ra[32], rb[32];
-        tmem_ld32(t_row + c0, ra);
-        tmem_ld32(t_row + BN / 2 + c0, rb);
-        tmem_ld_wait();
-#pragma unroll
-        for (int sub = 0; sub < 4; sub++) {
-          const uint32_t qq = tcount * CH + (c0 >> 3) + sub;
-          mbar_wait(afull_bar(quad, qq & 1), (qq >> 1) & 1);
-          const uint8_t* box = smem_al + (aff_buf - smem_base) + (qq & 1) * 4096 + lane * 128;
-          __align__(16) __half hi[8];
-          __align__(16) __half lo[8];
-          __align__(8) uint8_t h8[8];
-          __align__(8) uint8_t l8[8];
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            const float4 f = *reinterpret_cast<const float4*>(box + ((k ^ (lane & 7)) << 4));
-            const int i = sub * 8 + k;
-            float v = fmaxf(fmaf(f.x, __uint_as_float(ra[i]), f.y), 0.0f) + fmaxf(fmaf(f.z, __uint_as_float(rb[i]), f.w), 0.0f);
-            v *= a.act_scale;
-            const __half h = __float2half_rn(v);
-            const float hf = __half2float(h);
-            overflow |= valid && !(fabsf(hf) <= 65504.0f);
-            const float res = v - hf;
-            hi[k] = h;
-            lo[k] = __float2half_rn(res);
-            if (F8) {
-              h8[k] = to_e5m2(hf);
-              l8[k] = to_e5m2(res * af.scale_l8);
-            }
-          }
-          if (valid) {
-            *(uint4*)(a.out_hi + orow + c0 + sub * 8) = *(const uint4*)hi;
-            *(uint4*)(a.out_lo + orow + c0 + sub * 8) = *(const uint4*)lo;
-            if (F8) {
-              *(uint2*)(af.out_h8 + orow + c0 + sub * 8) = *(const uint2*)h8;
-              *(uint2*)(af.out_l8 + orow + c0 + sub * 8) = *(const uint2*)l8;
-            }
-          }
-          __syncwarp();
-          aff_issue(qq + 2);
-        }
-      }
-      if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(tempty_bar(acc) & PEER_MASK);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-  }
-}
-// -------------------------------------------------------------------------------------------------
-// Small nets (K = 64, boards up to 10x10: BASELINE config C2): the WHOLE network of one leaf in one CTA, one launch per
-// agent per MCTS wave instead of pack + init conv + one launch per block + head convs + heads (12+ launches of ~17 us:
-// the C2 wave was launch-bound, profiles/r01_bench_c2.json).  A 3x3 convolution mixes board points of ONE sample only, so
-// a CTA can carry a sample through every layer without any grid-wide step:
-//   * the sample's activations (128 + 2*(Wp+1) zero-bordered positions x 64 channels, fp16 hi/lo planes, SWIZZLE_128B
-//     rows) live in shared memory for the whole network; the epilogue of layer l writes layer l+1's operand in place,
-//     in the layout TMA would have produced (16-byte chunk index XOR row & 7), and the nine taps are row-shifted
-//     descriptor views of that one tile (see the halo kernel above);
-//   * only the filters stream (TMA, 2-stage ring that runs ahead across layer boundaries); tcgen05.mma cta_group::1,
-//     M = 128 (all positions of the sample), N = 64 (init conv) / 128 (both branches of a block), three fp16 passes in
-//     the same order as the layered kernels — the accumulators are bit-identical to the per-layer path;
-//   * the last block's epilogue feeds the two 1x1 head convolutions straight from registers; policy / value linears,
-//     softmax and tanh run on the CTA's epilogue warps (same summation order as k_head_convs_nhwc / k_heads_tiled).
-// 40 KB of activations + a 3-stage filter ring (96 KB, runs ahead across layers and samples) + 64 KB of staging for the
-// per-(point, channel) BN affine: 128 KB per layer and sample, four times the activations themselves — each epilogue warp
-// streams its 32 KB share in 8 KB chunks (cp.async.bulk, issued while the tensor core still works on the layer), so the
-// epilogue reads shared memory instead of stalling on L2 (ncu of the first version: 70 % of samples in long-scoreboard stalls).
-constexpr int SN_HR = 160;                       // activation rows: halo + 128 + halo, halo = Wp + 1 <= 16
-constexpr int SN_SLOTS = 2;                      // samples a CTA carries at once, one layer phase apart (tensor core on one
-                                                 // while the epilogue warps finish the other's previous layer)
-constexpr int SN_ACT_BYTES = 2 * SN_HR * 128;    // hi + lo planes of one slot
-constexpr int SN_NST = 3;                        // filter stages (96 KB in flight)
-constexpr int SN_WST_BYTES = 2 * 128 * 64 * 2;   // filter stage: hi + lo tiles of 128 rows x 64 K
-constexpr int SN_EPI_WARPS = 8;                  // two epilogue warps per TMEM lane quadrant: 32 channels each
-constexpr int SN_THREADS = 64 + 32 * SN_EPI_WARPS;
-constexpr int SN_CHUNK_CH = 4;                   // channels per staged affine chunk: 4 x 32 rows x float4 = 2 KB
-constexpr int SN_AFF_BYTES = SN_EPI_WARPS * 2 * 2048;
-constexpr int SN_SCRATCH = 16384;                // head-conv partial sums [128 rows][8 groups][3] + head vectors
-constexpr int SN_MAXL = 8;                       // init conv + up to 7 blocks
-__host__ __device__ constexpr int smem_bytes_small() {
-  return SN_SLOTS * SN_ACT_BYTES + SN_NST * SN_WST_BYTES + SN_AFF_BYTES + SN_SCRATCH + 1024 + 512;
-}
-
-struct SmallMaps { CUtensorMap hi[SN_MAXL], lo[SN_MAXL]; };
-struct SmallNetArgs {
-  const float* planes; const int* n_dev; int n_max;
-  int F, H, W, Wp, S, HW, A1, FC, nlayers /* init + blocks */, ldp;
-  float act_scale, inv_scale;
-  const float2* aff0;            // init layer {A', B}, laid out [row / 32][channel][row % 32] over the tile's 128 rows
-  const float* affq[SN_MAXL];    // blocks: {A'a, Ba, A'b, Bb}, same layout — a warp's load of one channel is 512 contiguous bytes
-  const float *wp, *gp, *bp, *wv, *gv, *bv;        // head convs (snapshot): filters [2][64] / [1][64], per-point gamma / beta
-  const float *pW, *pB, *vW, *vB, *voW, *voB;      // linears
-  float* policy; float* value; int* err;
-};
-__device__ __forceinline__ void bar_epi() { asm volatile("bar.sync 1, %0;" ::"n"(32 * SN_EPI_WARPS) : "memory"); }
-
-// Work items of a CTA, identical for the three roles: item w -> slot w & 1, step w >> 1 -> the slot's (step / nlayers)-th
-// sample = the CTA's sample number 2 (step / nlayers) + slot, layer step % nlayers.  Items of samples the CTA does not
-// have are skipped.
-struct SnItem { int slot, k, layer; bool exists; };
-__device__ __forceinline__ SnItem sn_item(uint32_t w, int nlayers, uint32_t my_samples) {
-  SnItem it;
-  it.slot = (int)(w & 1u);
-  const uint32_t step = w >> 1;
-  it.k = (int)(step / (uint32_t)nlayers) * 2 + it.slot;
-  it.layer = (int)(step % (uint32_t)nlayers);
-  it.exists = (uint32_t)it.k < my_samples;
-  return it;
-}
-
-// The filter stream is what the L2 has to feed: 32 KB per 768-clock K block per SM.  With 128 CTAs pipelined on two
-// samples each that is ~10 TB/s — the first pipelined version was bound by it (launch 122 us vs a 73 us MMA floor).  CTAs
-// therefore run as PAIRS (cluster of 2) on the same item sequence: rank 0 loads every stage's hi tile, rank 1 its lo tile,
-// each multicast into both CTAs' rings; a stage is refilled when both CTAs' tensor cores have consumed it (tcgen05.commit
-// multicast onto both empty barriers, count 2).  A pair whose CTAs own different sample counts pads the shorter one with
-// dummy items (zero input, nothing written).
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc2(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(SN_THREADS, 1)
-k_net_small(const __grid_constant__ SmallMaps maps, SmallNetArgs a) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
-  const uint32_t w_smem = smem_base + SN_SLOTS * SN_ACT_BYTES;
-  constexpr int AFF_OFF = SN_SLOTS * SN_ACT_BYTES + SN_NST * SN_WST_BYTES;
-  float* scratch = (float*)(smem_al + AFF_OFF + SN_AFF_BYTES);
-  const uint32_t bars = smem_base + AFF_OFF + SN_AFF_BYTES + SN_SCRATCH;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(smem_al + AFF_OFF + SN_AFF_BYTES + SN_SCRATCH + 448);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  auto wfull = [&](int s) { return bars + 8u * s; };
-  auto wempty = [&](int s) { return bars + 8u * (SN_NST + s); };
-  auto act_ready = [&](int slot) { return bars + 8u * (2 * SN_NST + slot); };
-  auto acc_full = [&](int slot) { return bars + 8u * (2 * SN_NST + 2 + slot); };
-  auto aff_bar = [&](int ew, int buf) { return bars + 8u * (2 * SN_NST + 4 + ew * 2 + buf); };
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < SN_NST; s++) { mbar_init(wfull(s), 1); mbar_init(wempty(s), 2); }  // empty: both CTAs of the pair
-    for (int sl = 0; sl < SN_SLOTS; sl++) { mbar_init(act_ready(sl), 32 * SN_EPI_WARPS); mbar_init(acc_full(sl), 1); }
-    for (int i = 0; i < 2 * SN_EPI_WARPS; i++) mbar_init(aff_bar(i >> 1, i & 1), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  // zero the activation tiles once: halo rows and the border positions stay zero for every sample and layer
-  for (int i = threadIdx.x; i < SN_SLOTS * SN_ACT_BYTES / 16; i += SN_THREADS) reinterpret_cast<uint4*>(smem_al)[i] = make_uint4(0, 0, 0, 0);
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // the peer's barriers are initialised before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  uint32_t crank;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(crank));
-  const int n = min(*a.n_dev, a.n_max);
-  const int halo = a.Wp + 1;
-  // effective grid: two samples per CTA (one per slot) whenever there are enough of them — the batch size is only known
-  // on the device, so the launch covers the SMs and the surplus CTAs leave at once
-  const int G = max(2, min((int)gridDim.x, (((n + 1) / 2) + 1) & ~1));  // even: CTAs work in pairs
-  auto samples_of = [&](int x) { return x < G && x < n ? (uint32_t)((n - x + G - 1) / G) : 0u; };
-  const uint32_t real_samples = samples_of((int)blockIdx.x);
-  // both CTAs of a pair walk the same item sequence (they share the filter stream): the longer list, the shorter padded
-  const uint32_t my_samples = max(real_samples, samples_of((int)(blockIdx.x ^ 1u)));
-  const uint32_t n_items = 2u * (uint32_t)a.nlayers * ((my_samples + 1u) / 2u);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== filter producer: streams every item's nine K blocks, ahead of the activations =====
-      uint32_t it = 0;
-      for (uint32_t w = 0; w < n_items; w++) {
-        const SnItem wi = sn_item(w, a.nlayers, my_samples);
-        if (!wi.exists) continue;
-        const int l = wi.layer;
-        const uint32_t bytes = l == 0 ? 2u * 64u * 64u * 2u : (uint32_t)SN_WST_BYTES;  // init conv: 64 filter rows
-        for (int tap = 0; tap < 9; tap++, it++) {
-          const int s = (int)(it % SN_NST);
-          mbar_wait(wempty(s), ((it / SN_NST) & 1u) ^ 1u);
-          const uint32_t sb = w_smem + s * SN_WST_BYTES;
-          mbar_expect_tx(wfull(s), bytes);  // own half + the peer's half, both land here
-          if (crank == 0) tma_load_2d_mc(sb, &maps.hi[l], wfull(s), tap * 64, 0, (uint16_t)3);
-          else tma_load_2d_mc(sb + 128 * 64 * 2, &maps.lo[l], wfull(s), tap * 64, 0, (uint16_t)3);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer: alternates between the two slots =====
-      uint32_t it = 0, cnt[SN_SLOTS] = {0, 0};
-      for (uint32_t w = 0; w < n_items; w++) {
-        const SnItem wi = sn_item(w, a.nlayers, my_samples);
-        if (!wi.exists) continue;
-        const int l = wi.layer, sl = wi.slot;
-        mbar_wait(act_ready(sl), cnt[sl] & 1u);
-        cnt[sl]++;
-        tc_fence_after();
-        const uint32_t idesc = l == 0 ? make_idesc(BM, 64) : make_idesc(BM, 128);
-        const uint32_t act_hi = smem_base + sl * SN_ACT_BYTES, act_lo = act_hi + SN_HR * 128;
-        const uint32_t d_tmem = tmem_base + sl * 128;
-        for (int tap = 0; tap < 9; tap++, it++) {
-          const int s = (int)(it % SN_NST);
-          mbar_wait(wfull(s), (it / SN_NST) & 1u);
-          tc_fence_after();
-          const int dy = tap / 3 - 1, dx = tap - (tap / 3) * 3 - 1;
-          const uint32_t j0 = (uint32_t)(halo + dy * a.Wp + dx);
-          const uint32_t sb = w_smem + s * SN_WST_BYTES;
-          const uint64_t dAh = make_desc_sw<64>(act_hi + j0 * 128u), dAl = make_desc_sw<64>(act_lo + j0 * 128u);
-          const uint64_t dBh = make_desc_sw<64>(sb), dBl = make_desc_sw<64>(sb + 128 * 64 * 2);
-#pragma unroll
-          for (int ks = 0; ks < 4; ks++) {
-            const uint64_t adv = (uint64_t)(ks * 2);
-            umma_f16(d_tmem, dAh + adv, dBh + adv, idesc, (tap | ks) ? 1u : 0u);
-            umma_f16(d_tmem, dAh + adv, dBl + adv, idesc, 1u);
-            umma_f16(d_tmem, dAl + adv, dBh + adv, idesc, 1u);
-          }
-          umma_commit_mc2(wempty(s));  // the stage is free once both CTAs of the pair have read it
-        }
-        umma_commit(acc_full(sl));
-      }
-    }
-  } else {
-    // ===== epilogue warps: thread = (board position = TMEM lane, half of the channels) =====
-    const int ew = warp - 2;                        // 0..7
-    const int quad = warp & 3, half = ew >> 2;      // TMEM lane quadrant = warp % 4; channels [32 half, 32 half + 32)
-    const int r = quad * 32 + lane;                 // position inside the sample's tile
-    const int y = r / a.Wp, x = r - y * a.Wp;
-    const bool valid = r < a.S && y < a.H && x < a.W;
-    const int hw = y * a.W + x;
-    const uint32_t brow = (uint32_t)(halo + r);
-    const int epi_tid = threadIdx.x - 64;           // 0..255
-    float* s_part = scratch;                        // [128 rows][8 channel groups][3]: head-conv partial sums
-    float* s_ph = scratch + 128 * 8 * 3;            // [2*HW]
-    float* s_vh = s_ph + 2 * a.HW;                  // [HW]
-    float* s_lg = s_vh + a.HW;                      // [A1]
-    float* s_hh = s_lg + a.A1;                      // [FC]
-    bool nanflag = false;
-    float amax = 0.0f;
-    // ---- staged affine: chunks of 4 channels, consumed in item order; the issue cursor runs two chunks ahead
-    constexpr int CPL = 32 / SN_CHUNK_CH;           // chunks per layer for this warp
-    const uint32_t aff_buf = smem_base + AFF_OFF + ew * 4096;
-    const uint8_t* aff_ptr = smem_al + AFF_OFF + ew * 4096;
-    uint32_t qq_issue = 0, qq_use = 0, w_issue = 0;
-    int part_issue = 0;
-    while (w_issue < n_items && !sn_item(w_issue, a.nlayers, my_samples).exists) w_issue++;
-    auto aff_issue = [&]() {
-      if (w_issue >= n_items) return;
-      const int l = sn_item(w_issue, a.nlayers, my_samples).layer;
-      const uint32_t bytes = l == 0 ? 1024u : 2048u;  // float2 / float4 per (channel, row)
-      if (lane == 0) {
-        const uint8_t* src = l == 0 ? reinterpret_cast<const uint8_t*>(a.aff0) : reinterpret_cast<const uint8_t*>(a.affq[l]);
-        src += ((size_t)quad * 64 + half * 32 + part_issue * SN_CHUNK_CH) * 32 * (l == 0 ? 8 : 16);
-        const uint32_t bar = aff_bar(ew, (int)(qq_issue & 1u));
-        mbar_expect_tx(bar, bytes);
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(aff_buf + (qq_issue & 1u) * 2048u), "l"(src), "r"(bytes), "r"(bar) : "memory");
-      }
-      qq_issue++;
-      if (++part_issue == CPL) {
-        part_issue = 0;
-        w_issue++;
-        while (w_issue < n_items && !sn_item(w_issue, a.nlayers, my_samples).exists) w_issue++;
-      }
-    };
-    aff_issue();
-    aff_issue();
-    // the encoder's planes of the CTA's k-th sample -> the slot's first operand (k_pack_planes' arithmetic)
-    auto load_planes = [&](int k) {
-      const int sl = k & 1;
-      const int b = (int)blockIdx.x + k * G;
-      uint8_t* row_hi = smem_al + (size_t)sl * SN_ACT_BYTES + (size_t)brow * 128;
-      uint8_t* row_lo = row_hi + (size_t)SN_HR * 128;
-#pragma unroll 1
-      for (int cc = half * 4; cc < half * 4 + 4; cc++) {
-        __align__(16) __half hi[8];
-        __align__(16) __half lo[8];
-#pragma unroll
-        for (int kk = 0; kk < 8; kk++) {
-          const int c = cc * 8 + kk;
-          const float v = (valid && c < a.F && (uint32_t)k < real_samples) ? a.planes[((size_t)b * a.F + c) * a.HW + hw] * a.act_scale : 0.0f;
-          const __half h = __float2half_rn(v);
-          hi[kk] = h;
-          lo[kk] = __float2half_rn(v - __half2float(h));
-        }
-        const uint32_t off = (uint32_t)((cc ^ (int)(brow & 7u)) << 4);
-        *reinterpret_cast<uint4*>(row_hi + off) = *reinterpret_cast<const uint4*>(hi);
-        *reinterpret_cast<uint4*>(row_lo + off) = *reinterpret_cast<const uint4*>(lo);
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      mbar_arrive(act_ready(sl));
-    };
-    if (my_samples > 0) load_planes(0);
-    if (my_samples > 1) load_planes(1);
-    uint32_t acnt[SN_SLOTS] = {0, 0};
-    for (uint32_t w = 0; w < n_items; w++) {
-      const SnItem wi = sn_item(w, a.nlayers, my_samples);
-      if (!wi.exists) continue;
-      const int l = wi.layer, sl = wi.slot;
-      const int b = (int)blockIdx.x + wi.k * G;
-      const bool last = l == a.nlayers - 1;
-      uint8_t* row_hi = smem_al + (size_t)sl * SN_ACT_BYTES + (size_t)brow * 128;
-      uint8_t* row_lo = row_hi + (size_t)SN_HR * 128;
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + sl * 128 + half * 32;
-      mbar_wait(acc_full(sl), acnt[sl] & 1u);
-      acnt[sl]++;
-      tc_fence_after();
-      uint32_t ra[32], rb[32];
-      tmem_ld32(t_row, ra);
-      if (l > 0) tmem_ld32(t_row + 64, rb);
-      tmem_ld_wait();
-#pragma unroll
-      for (int sub = 0; sub < 4; sub++) {  // 8 channels = one 16-byte operand chunk = two staged affine chunks
-        __align__(16) __half2 hi2[4];
-        __align__(16) __half2 lo2[4];
-        const int cbase = half * 32 + sub * 8;
-        float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f;
-#pragma unroll
-        for (int hc = 0; hc < 2; hc++) {
-          mbar_wait(aff_bar(ew, (int)(qq_use & 1u)), (qq_use >> 1) & 1u);
-          const uint8_t* chunk = aff_ptr + (qq_use & 1u) * 2048u;
-          float v[4];
-#pragma unroll
-          for (int kk = 0; kk < 4; kk++) {
-            const int i = sub * 8 + hc * 4 + kk;
-            // the staged affine already carries the activation scale 2^ea (exact) and is all-zero on border / padding
-            // rows, so neither a multiply nor a validity select is needed here
-            if (l == 0) {
-              const float2 fa = reinterpret_cast<const float2*>(chunk)[kk * 32 + lane];
-              v[kk] = fmaxf(fmaf(fa.x, __uint_as_float(ra[i]), fa.y), 0.0f);
-            } else {
-              const float4 f = reinterpret_cast<const float4*>(chunk)[kk * 32 + lane];
-              v[kk] = fmaxf(fmaf(f.x, __uint_as_float(ra[i]), f.y), 0.0f) + fmaxf(fmaf(f.z, __uint_as_float(rb[i]), f.w), 0.0f);
-            }
-            amax = fmaxf(amax, v[kk]);  // v >= 0; NaN / inf reach the overflow check through the fp16 conversion below
-          }
-#pragma unroll
-          for (int pr = 0; pr < 2; pr++) {
-            const __half2 h2 = __floats2half2_rn(v[2 * pr], v[2 * pr + 1]);
-            const float2 hf = __half22float2(h2);
-            const __half2 l2 = __floats2half2_rn(v[2 * pr] - hf.x, v[2 * pr + 1] - hf.y);
-            hi2[hc * 2 + pr] = h2; lo2[hc * 2 + pr] = l2;
-            nanflag |= !(hf.x <= 65504.0f) || !(hf.y <= 65504.0f);
-            if (last) {  // the 1x1 head convolutions read what the layered path would have stored: (hi + lo) / scale
-              const float2 lf = __half22float2(l2);
-              const int ch = cbase + hc * 4 + 2 * pr;
-              const float vv0 = (hf.x + lf.x) * a.inv_scale, vv1 = (hf.y + lf.y) * a.inv_scale;
-              a0 = fmaf(vv0, __ldg(a.wp + ch), a0);      a0 = fmaf(vv1, __ldg(a.wp + ch + 1), a0);
-              a1 = fmaf(vv0, __ldg(a.wp + 64 + ch), a1); a1 = fmaf(vv1, __ldg(a.wp + 64 + ch + 1), a1);
-              a2 = fmaf(vv0, __ldg(a.wv + ch), a2);      a2 = fmaf(vv1, __ldg(a.wv + ch + 1), a2);
-            }
-          }
-          qq_use++;
-          __syncwarp();  // chunk consumed by every lane: refill its buffer with the chunk after next
-          aff_issue();
-        }
-        if (last) {
-          float* o = s_part + ((size_t)r * 8 + (cbase >> 3)) * 3;
-          o[0] = a0; o[1] = a1; o[2] = a2;
-        } else {
-          const uint32_t off = (uint32_t)(((cbase >> 3) ^ (int)(brow & 7u)) << 4);
-          *reinterpret_cast<uint4*>(row_hi + off) = *reinterpret_cast<const uint4*>(hi2);
-          *reinterpret_cast<uint4*>(row_lo + off) = *reinterpret_cast<const uint4*>(lo2);
-        }
-      }
-      tc_fence_before();
-      if (!last) {
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive(act_ready(sl));
-      } else {
-        // ---- heads.  Head convs: the xor-shuffle tree of k_head_convs_nhwc over its lanes 0..7 (8 channels each)
-        bar_epi();
-        if (valid && half == 0) {
-          const float* q = s_part + (size_t)r * 24;
-          const float isd = 1.0f / sqrtf(1e-5f);
-          const float q0 = ((q[0] + q[12]) + (q[6] + q[18])) + ((q[3] + q[15]) + (q[9] + q[21]));
-          const float q1 = ((q[1] + q[13]) + (q[7] + q[19])) + ((q[4] + q[16]) + (q[10] + q[22]));
-          const float q2 = ((q[2] + q[14]) + (q[8] + q[20])) + ((q[5] + q[17]) + (q[11] + q[23]));
-          const float p0 = a.gp[hw] * (q0 * isd) + a.bp[hw];
-          const float p1 = a.gp[a.HW + hw] * (q1 * isd) + a.bp[a.HW + hw];
-          const float v0 = a.gv[hw] * (q2 * isd) + a.bv[hw];
-          s_ph[hw] = p0 > 0.0f ? p0 : 0.0f;
-          s_ph[a.HW + hw] = p1 > 0.0f ? p1 : 0.0f;
-          s_vh[hw] = v0 > 0.0f ? v0 : 0.0f;
-        }
-        bar_epi();
-        const int J2 = 2 * a.HW;
-        for (int o = epi_tid; o < a.A1 + a.FC; o += 32 * SN_EPI_WARPS) {   // k_heads_tiled: ascending-j fma chains
-          if (o < a.A1) {
-            float acc = 0.0f;
-#pragma unroll 27
-            for (int j = 0; j < J2; j++) acc = fmaf(s_ph[j], __ldg(a.pW + (size_t)j * a.A1 + o), acc);
-            s_lg[o] = expf(acc + a.pB[o]);
-          } else {
-            const int f = o - a.A1;
-            float acc = 0.0f;
-#pragma unroll 27
-            for (int j = 0; j < a.HW; j++) acc = fmaf(s_vh[j], __ldg(a.vW + (size_t)j * a.FC + f), acc);
-            const float v = acc + a.vB[f];
-            s_hh[f] = v > 0.0f ? v : 0.0f;
-          }
-        }
-        bar_epi();
-        if (epi_tid < 32 && (uint32_t)wi.k < real_samples) {
-          float sum = 0.0f, dot = 0.0f;
-          for (int o = lane; o < a.A1; o += 32) sum += s_lg[o];
-          for (int f = lane; f < a.FC; f += 32) dot = fmaf(s_hh[f], a.voW[f], dot);
-#pragma unroll
-          for (int off = 16; off; off >>= 1) { sum += __shfl_xor_sync(0xffffffffu, sum, off); dot += __shfl_xor_sync(0xffffffffu, dot, off); }
-          for (int o = lane; o < a.A1; o += 32) a.policy[(size_t)b * a.ldp + o] = s_lg[o] / sum;
-          if (lane == 0) a.value[b] = tanhf(dot + a.voB[0]);
-        }
-        bar_epi();  // the scratch is free for the other slot's heads
-        if ((uint32_t)(wi.k + 2) < my_samples) load_planes(wi.k + 2);  // the slot's next sample
-      }
-    }
-    if (nanflag || !(amax <= 65504.0f)) atomicOr(a.err, ERR_ACT_OVERFLOW);
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // nobody leaves while the peer may still multicast into this CTA's ring or signal its barriers
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256));
-  }
-}
-
-// (hi16, lo16) -> (e4m3(hi * 2^pa), e4m3(lo * 2^q)) for the rows a non-fp8 kernel produced (the init conv's output)
-__global__ void k_split_fp8(const __half* __restrict__ hi, const __half* __restrict__ lo, size_t n, float scale_h8, float scale_l8,
-                            uint8_t* h8, uint8_t* l8) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  h8[i] = to_e5m2(__half2float(hi[i]) * scale_h8);
-  l8[i] = to_e5m2(__half2float(lo[i]) * scale_l8);
-}
 
 // fp32 NCHW planes -> zero-bordered NHWC fp16 hi/lo (channels padded to cpad)
 __global__ void k_pack_planes(const float* __restrict__ planes, const int* __restrict__ n_dev, int n_max, int F, int H,
@@ -1282,75 +87,187 @@ __global__ void k_head_convs_nhwc(const __half* __restrict__ hi, const __half* _
   }
 }
 
-// dynamic shared memory opt-in of every instantiation this file launches, on the current device (the attribute is per
-// function and per device; called from the allocator, which runs with the engine's device current)
-template <int BN, bool PAIR, int BKT>
-void set_conv_attr() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, BKT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN, BKT, PAIR)));
-}
-void tower_configure_device() {
-  set_conv_attr<256, true, 64>(); set_conv_attr<128, true, 64>(); set_conv_attr<256, false, 64>(); set_conv_attr<128, false, 64>();
-  set_conv_attr<64, false, 64>();
-  set_conv_attr<256, true, 32>(); set_conv_attr<128, true, 32>(); set_conv_attr<256, false, 32>(); set_conv_attr<128, false, 32>();
-  set_conv_attr<64, false, 32>();
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes2()));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc2_f8, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes2()));
-  CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small()));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc2_halo<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_f8h(F8H_MAX_HROWS)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc2_halo<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_f8h(F8H_MAX_HROWS)));
+// -------------------------------------------------------------------------------------------------
+// k_net_small: the whole tower of a K = 64 net on a board of at most 128 padded positions ((H+1)(W+1) <= 128, BASELINE
+// C2) in one persistent kernel.  A 3x3 convolution mixes board points of one sample only, so a CTA carries a sample
+// through every layer with no grid-wide step: the sample's zero-bordered positions x 64 channels stay in shared memory as
+// fp16 hi / lo planes (two ping-pong buffers), only the filters stream from L2 (TMA into an mbarrier ring that runs ahead
+// across layers and samples, one stage per (layer, tap)), and the last layer writes the NHWC hi/lo buffer the head
+// kernels read.  Activations are stored K-major without swizzle ([8-channel chunk][row][16 B]), so tap (dy, dx) is the
+// same tile with its descriptor starting dy*(W+1)+dx rows further — no copy per tap.  Same MMA sequence (tap by tap, three
+// passes), same epilogue arithmetic as the per-layer kernels: the outputs are identical to that path.
+constexpr int SN_MAXL = 8;                 // init conv + up to 7 blocks
+constexpr int SN_R0 = 16;                  // halo rows in front of the tile (>= W + 2)
+constexpr int SN_HR = 160;                 // rows per activation plane: halo + 128 + halo
+constexpr int SN_PLANE = 8 * SN_HR * 16;   // one fp16 plane: 8 chunks of 8 channels x SN_HR rows x 16 B
+constexpr int SN_NST = 4;                  // filter stages
+constexpr int SN_STAGE = 2 * 128 * BK * 2; // hi + lo filter tiles of up to 128 rows x 64 K
+__host__ __device__ constexpr int smem_bytes_small() { return 4 * SN_PLANE + SN_NST * SN_STAGE + 1024 + 256; }
+struct SmallMaps { CUtensorMap hi[SN_MAXL], lo[SN_MAXL]; };
+struct SmallNetArgs {
+  const float* planes;  // [n][F][HW] encoder planes
+  const int* n_dev;
+  int n_max, F, H, W, Wp, S, HW, nlayers, guard, passes;
+  float act_scale;
+  const float2* aff[SN_MAXL];  // per layer [HW][n_total] {A', B}
+  __half *out_hi, *out_lo;     // last layer: [(guard + n*S)][64], the layout k_head_convs_nhwc reads
+  int* err;
+};
+
+// one layer of one sample: 9 taps of the filter ring into acc, then the epilogue into smem (or global for the last layer)
+template <int N>
+__device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int smp, uint32_t act, uint32_t ring, uint32_t bars,
+                                            uint32_t& it, int in, bool& overflow) {
+  constexpr bool PAIR = N == 128;
+  constexpr int OUTC = PAIR ? N / 2 : N;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+  const uint32_t in_hi = act + (2 * in) * SN_PLANE, in_lo = in_hi + SN_PLANE;
+  float acc[N / 2];
+  for (int tap = 0; tap < 9; tap++, it++) {
+    const int st = it % SN_NST;
+    mbar_wait(bars + 8u * st, (it / SN_NST) & 1);
+    __syncwarp();
+    const uint32_t shift = (uint32_t)(SN_R0 + wg * 64 + (tap / 3 - 1) * a.Wp + (tap % 3 - 1)) * 16;
+    const uint32_t sb = ring + st * SN_STAGE;
+    mma_kblock<N, 0>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_lo + shift, SN_HR * 16),
+                     make_desc_sw(sb), make_desc_sw(sb + SN_STAGE / 2), 32 >> 4, tap == 0, a.passes, 2 * SN_HR * 16 >> 4);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bars + 8u * (SN_NST + st));
+  }
+  const bool last = l == a.nlayers - 1;
+  const uint32_t out_hi = act + (2 * (in ^ 1)) * SN_PLANE, out_lo = out_hi + SN_PLANE;
+  const int n_total = PAIR ? 128 : 64;
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int p = row0 + 8 * h;  // position inside the sample
+    const int y = p / a.Wp, x = p - y * a.Wp;
+    const bool valid = p < a.S && y < a.H && x < a.W;
+    if (last && !valid) continue;
+    const float2* aff = a.aff[l] + (size_t)(valid ? y * a.W + x : 0) * n_total + col0;
+    const size_t grow = (size_t)a.guard + (size_t)smp * a.S + p;
+#pragma unroll
+    for (int j = 0; j < OUTC / 8; j++) {
+      __half hv[2], lv[2];
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        float v = 0.0f;
+        if (valid) {
+          const float2 fa = __ldg(aff + 8 * j + e);
+          v = fmaxf(fmaf(fa.x, acc[4 * j + 2 * h + e], fa.y), 0.0f);
+          if (PAIR) {
+            const float2 fb = __ldg(aff + N / 2 + 8 * j + e);
+            v += fmaxf(fmaf(fb.x, acc[4 * (j + OUTC / 8) + 2 * h + e], fb.y), 0.0f);
+          }
+          v *= a.act_scale;
+        }
+        const __half hh = __float2half_rn(v);
+        const float hf = __half2float(hh);
+        overflow |= !(fabsf(hf) <= 65504.0f);
+        hv[e] = hh;
+        lv[e] = __float2half_rn(v - hf);
+      }
+      const int c = 8 * j + col0;
+      if (last) {
+        *reinterpret_cast<__half2*>(a.out_hi + grow * 64 + c) = __halves2half2(hv[0], hv[1]);
+        *reinterpret_cast<__half2*>(a.out_lo + grow * 64 + c) = __halves2half2(lv[0], lv[1]);
+      } else {  // chunk c / 8, row SN_R0 + p, byte (c % 8) * 2; invalid positions are written as zeros
+        const uint32_t o = (uint32_t)(c >> 3) * (SN_HR * 16) + (uint32_t)(SN_R0 + p) * 16 + (uint32_t)(c & 7) * 2;
+        const __half2 h2 = __halves2half2(hv[0], hv[1]), l2 = __halves2half2(lv[0], lv[1]);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_hi + o), "r"(*reinterpret_cast<const uint32_t*>(&h2)) : "memory");
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_lo + o), "r"(*reinterpret_cast<const uint32_t*>(&l2)) : "memory");
+      }
+    }
+  }
 }
 
-// 1-byte operands (FP8 correction passes): [rows][cols] bytes, box {64 bytes, box_rows}, SWIZZLE_64B
-CUtensorMap make_map_u8(void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
-  CUtensorMap m;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols};
-  cuuint32_t box[2] = {64, box_rows};
-  cuuint32_t es[2] = {1, 1};
-  CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(u8) failed: " + std::to_string((int)r));
-  return m;
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+__global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant__ SmallMaps maps, SmallNetArgs a) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
+  const uint32_t act = base;                     // 4 planes: buffer b hi at 2b, lo at 2b + 1
+  const uint32_t ring = base + 4 * SN_PLANE;      // filter stages (1024-aligned: SN_PLANE is a multiple of 1024)
+  const uint32_t bars = ring + SN_NST * SN_STAGE; // full[NST], empty[NST]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int i = threadIdx.x; i < 4 * SN_PLANE / 16; i += blockDim.x) reinterpret_cast<uint4*>(base_ptr)[i] = make_uint4(0, 0, 0, 0);
+  if (threadIdx.x == 0) {
+    for (int st = 0; st < SN_NST; st++) { mbar_init(bars + 8u * st, 1); mbar_init(bars + 8u * (SN_NST + st), CONSUMER_WARPS); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  proxy_fence();  // the zeroed halo rows are read by wgmma
+  __syncthreads();
+  const int n = min(*a.n_dev, a.n_max);
+  if (warp == PRODUCER_WARP) {
+    if (lane == 0) {
+      uint32_t it = 0;
+      for (int smp = blockIdx.x; smp < n; smp += gridDim.x)
+        for (int l = 0; l < a.nlayers; l++) {
+          const uint32_t bytes = 2u * (l == 0 ? 64 : 128) * BK * 2;
+          for (int tap = 0; tap < 9; tap++, it++) {
+            const int st = it % SN_NST;
+            mbar_wait(bars + 8u * (SN_NST + st), ((it / SN_NST) & 1) ^ 1);
+            const uint32_t sb = ring + st * SN_STAGE;
+            mbar_expect_tx(bars + 8u * st, bytes);
+            tma_load_2d(sb, &maps.hi[l], bars + 8u * st, tap * BK, 0);
+            tma_load_2d(sb + SN_STAGE / 2, &maps.lo[l], bars + 8u * st, tap * BK, 0);
+          }
+        }
+    }
+    return;
+  }
+  const int tid = threadIdx.x;  // 0..255: the two consumer warpgroups
+  uint32_t it = 0;
+  bool overflow = false;
+  for (int smp = blockIdx.x; smp < n; smp += gridDim.x) {
+    // encoder planes -> buffer 0 (the same values k_pack_planes writes for the per-layer path)
+    for (int i = tid; i < 128 * 64; i += 256) {
+      const int p = i >> 6, c = i & 63;
+      const int y = p / a.Wp, x = p - y * a.Wp;
+      float v = 0.0f;
+      if (p < a.S && y < a.H && x < a.W && c < a.F) v = a.planes[((size_t)smp * a.F + c) * a.HW + y * a.W + x] * a.act_scale;
+      const __half h = __float2half_rn(v);
+      const uint32_t o = (uint32_t)(c >> 3) * (SN_HR * 16) + (uint32_t)(SN_R0 + p) * 16 + (uint32_t)(c & 7) * 2;
+      *reinterpret_cast<__half*>(base_ptr + o) = h;
+      *reinterpret_cast<__half*>(base_ptr + SN_PLANE + o) = __float2half_rn(v - __half2float(h));
+    }
+    proxy_fence();
+    consumer_sync();
+    for (int l = 0; l < a.nlayers; l++) {
+      if (l == 0) small_layer<64>(a, l, smp, act, ring, bars, it, 0, overflow);
+      else small_layer<128>(a, l, smp, act, ring, bars, it, l & 1, overflow);
+      proxy_fence();   // this layer's generic smem writes are read by the next layer's wgmma (async proxy)
+      consumer_sync(); // and every warp's MMAs on the buffer the next layer overwrites have completed
+    }
+  }
+  if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
 }
-CUtensorMap make_map3d_u8(void* base, uint64_t n, uint64_t S, uint64_t cols, uint32_t box_rows = BM) {
-  CUtensorMap m;
-  cuuint64_t dims[3] = {cols, S, n};
-  cuuint64_t strides[2] = {cols, S * cols};
-  cuuint32_t box[3] = {64, box_rows, 1};
-  cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(u8, 3d) failed: " + std::to_string((int)r));
-  return m;
+
+// dynamic shared memory opt-in of every instantiation this file launches, on the current device (the attribute is per
+// function and per device; called from the allocator, which runs with the engine's device current)
+template <int BN, bool PAIR>
+void set_conv_attr() {
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN)));
+}
+void tower_configure_device() {
+  set_conv_attr<256, true>(); set_conv_attr<128, true>(); set_conv_attr<256, false>(); set_conv_attr<128, false>();
+  set_conv_attr<64, false>();
+  CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small()));
 }
 
 struct Layer {
   int cin, n_total, bn;
   bool pair;
   __half *w_hi = nullptr, *w_lo = nullptr;  // [n_total][9*cin]
-  float2* aff = nullptr;                    // [HW][n_total]  (single layers: read by the epilogue with global loads)
-  float* affq = nullptr;                    // fused pairs: [aff_rows][K] x {A'a, Ba, A'b, Bb}, rows = positions in layout order
-  int aff_rows = 0;
-  CUtensorMap mB_hi, mB_lo, mAff;
-  CUtensorMap mB2_hi, mB2_lo;               // CTA-pair kernel: 128-row boxes (each CTA of the pair loads half of the N tile)
-  float* affs = nullptr;                    // k_net_small: the layer's affine as [4][64][32] x (float2 | float4), rows = tile positions
-  // FP8 correction passes (AZ_FLAG_FAST_TOWER): e4m3(w_hi * 2^-q), e4m3(w_lo * 2^-pa), 64-byte-row boxes
-  uint8_t *w_h8 = nullptr, *w_l8 = nullptr;
-  CUtensorMap mB2_h8, mB2_l8;
+  float2* aff = nullptr;                    // [HW][n_total] {A', B} in weight-row order
+  CUtensorMap mB_hi, mB_lo;
 };
 struct Impl {
   NetDims d;
-  int n_max, ea, guard, S, rows_alloc, num_sms, passes = 3, mode3d = 0, tps = 1, bk = 64;
-  int pair_clusters = 0;  // > 0: fused layers run on k_conv3x3_tc2 with this many co-resident CTA pairs
-  // correction passes on the FP8 tensor path (AZ_FLAG_FAST_TOWER); activations then also travel as e5m2 h8 / l8
-  int fp8 = 0;         // 0: three fp16 passes; 1: per-tap FP8-correction kernel (A/B); 2: halo FP8-correction kernel (default)
-  int pa = 0, q = 11;  // h8 = e5m2(hi16 * 2^pa), l8 = e5m2(lo * 2^q); filters (e4m3) carry the inverse factors
-  int hrows = 0, halo = 0;                     // halo kernel: rows per activation stage, Wp + 1
-  bool halo3 = false;                          // three fp16 passes on the halo pipeline (the fp32-faithful default)
-  bool small = false;                          // K = 64, board <= 10x10: the whole network in one kernel (k_net_small)
-  CUtensorMap mXh_hi[2], mXh_lo[2], mXh_h8[2], mXh_l8[2];  // halo boxes {64 channels, hrows positions}
-  uint8_t *x_h8[2] = {nullptr, nullptr}, *x_l8[2] = {nullptr, nullptr};
-  CUtensorMap mX_h8[2], mX_l8[2];
+  int n_max, ea, guard, S, rows_alloc, num_sms, passes = 3, mode3d = 0, tps = 1;
+  bool small = false;  // K = 64, (H+1)(W+1) <= 128: the whole tower of a sample in one kernel (k_net_small)
   __half *xin_hi = nullptr, *xin_lo = nullptr;  // [(guard+rows+guard)][64]
   __half *x_hi[2] = {nullptr, nullptr}, *x_lo[2] = {nullptr, nullptr};  // [(guard+rows+guard)][K]
   CUtensorMap mIn_hi, mIn_lo, mX_hi[2], mX_lo[2];
@@ -1367,7 +284,7 @@ struct Impl {
   }
 };
 
-template <int BN, bool PAIR, int BKT>
+template <int BN, bool PAIR>
 void launch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
                  const int* n_dev, int* err, cudaStream_t st) {
   ConvArgs a;
@@ -1378,74 +295,16 @@ void launch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUt
   a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
   const int max_tiles = (I.mode3d ? I.n_max * I.tps : (I.n_max * I.S + BM - 1) / BM) * (L.n_total / BN);
   const int grid = std::min(I.num_sms, max_tiles);
-  k_conv3x3_tc<BN, PAIR, BKT><<<grid, NTHREADS, smem_bytes(BN, BKT, PAIR), st>>>(ah, al, L.mB_hi, L.mB_lo, PAIR ? L.mAff : L.mB_hi, a); LAUNCH_CHECK();
-}
-template <int BKT>
-void dispatch_conv_bk(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
-                      const int* n_dev, int* err, cudaStream_t st) {
-  if (L.pair && L.bn == 256) launch_conv<256, true, BKT>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (L.pair && L.bn == 128) launch_conv<128, true, BKT>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (!L.pair && L.bn == 256) launch_conv<256, false, BKT>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (!L.pair && L.bn == 128) launch_conv<128, false, BKT>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (!L.pair && L.bn == 64) launch_conv<64, false, BKT>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else throw std::runtime_error("tc tower: unsupported tile");
-}
-void launch_conv_pair2(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
-                       const int* n_dev, int* err, cudaStream_t st) {
-  ConvArgs a;
-  a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
-  a.mode3d = I.mode3d; a.tps = I.tps;
-  a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff; a.out_hi = ohi; a.out_lo = olo;
-  a.act_scale = ldexpf(1.0f, I.ea); a.err = err; a.passes = I.passes;
-  a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
-  const int m_tiles = I.mode3d ? I.n_max * I.tps : (I.n_max * I.S + BM - 1) / BM;
-  const int pair_tiles = ((m_tiles + 1) / 2) * (L.n_total / 256);
-  const int clusters = std::min(I.pair_clusters, pair_tiles);
-  k_conv3x3_tc2<<<2 * clusters, NTHREADS, smem_bytes2(), st>>>(ah, al, L.mB2_hi, L.mB2_lo, L.mAff, a); LAUNCH_CHECK();
-}
-void launch_conv_pair2_f8(const Impl& I, const Layer& L, int in, int out, const int* n_dev, int* err, cudaStream_t st) {
-  ConvArgsF8 af;
-  ConvArgs& a = af.c;
-  a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
-  a.mode3d = I.mode3d; a.tps = I.tps;
-  a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff; a.out_hi = I.x_hi[out]; a.out_lo = I.x_lo[out];
-  a.act_scale = ldexpf(1.0f, I.ea); a.err = err; a.passes = 3;
-  a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
-  af.out_h8 = I.x_h8[out]; af.out_l8 = I.x_l8[out];
-  af.scale_h8 = ldexpf(1.0f, I.pa); af.scale_l8 = ldexpf(1.0f, I.q);
-  const int m_tiles = I.mode3d ? I.n_max * I.tps : (I.n_max * I.S + BM - 1) / BM;
-  const int pair_tiles = ((m_tiles + 1) / 2) * (L.n_total / 256);
-  const int clusters = std::min(I.pair_clusters, pair_tiles);
-  k_conv3x3_tc2_f8<<<2 * clusters, NTHREADS, smem_bytes2(), st>>>(I.mX_hi[in], I.mX_h8[in], I.mX_l8[in], L.mB2_hi, L.mB2_h8,
-                                                                  L.mB2_l8, L.mAff, af); LAUNCH_CHECK();
-}
-void launch_conv_pair2_f8h(const Impl& I, const Layer& L, int in, int out, const int* n_dev, int* err, cudaStream_t st) {
-  ConvArgsF8H af;
-  ConvArgs& a = af.c;
-  a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
-  a.mode3d = I.mode3d; a.tps = I.tps;
-  a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff; a.out_hi = I.x_hi[out]; a.out_lo = I.x_lo[out];
-  a.act_scale = ldexpf(1.0f, I.ea); a.err = err; a.passes = 3;
-  a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
-  af.out_h8 = I.x_h8[out]; af.out_l8 = I.x_l8[out];
-  af.scale_l8 = ldexpf(1.0f, I.q);
-  af.hrows = I.hrows; af.halo = I.halo;
-  const int m_tiles = I.mode3d ? I.n_max * I.tps : (I.n_max * I.S + BM - 1) / BM;
-  const int pair_tiles = ((m_tiles + 1) / 2) * (L.n_total / 256);
-  const int clusters = std::min(I.pair_clusters, pair_tiles);
-  if (I.fp8 == 2)
-    k_conv3x3_tc2_halo<true><<<2 * clusters, NTHREADS, smem_bytes_f8h(I.hrows), st>>>(I.mXh_hi[in], I.mXh_h8[in], I.mXh_l8[in], L.mB2_hi,
-                                                                                   L.mB2_h8, L.mB2_l8, L.mAff, af);
-  else  // three fp16 passes on the halo pipeline
-    k_conv3x3_tc2_halo<false><<<2 * clusters, NTHREADS, smem_bytes_f8h(I.hrows), st>>>(I.mXh_hi[in], I.mXh_lo[in], I.mXh_lo[in], L.mB2_hi,
-                                                                                    L.mB2_lo, L.mB2_lo, L.mAff, af);
-  LAUNCH_CHECK();
+  k_conv3x3_tc<BN, PAIR><<<grid, NTHREADS, smem_bytes(BN), st>>>(ah, al, L.mB_hi, L.mB_lo, a); LAUNCH_CHECK();
 }
 void dispatch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
                    const int* n_dev, int* err, cudaStream_t st) {
-  if (I.pair_clusters > 0 && L.pair && L.bn == 256) launch_conv_pair2(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (I.bk == 64) dispatch_conv_bk<64>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else dispatch_conv_bk<32>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  if (L.pair && L.bn == 256) launch_conv<256, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (L.pair && L.bn == 128) launch_conv<128, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (!L.pair && L.bn == 256) launch_conv<256, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (!L.pair && L.bn == 128) launch_conv<128, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (!L.pair && L.bn == 64) launch_conv<64, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else throw std::runtime_error("tc tower: unsupported tile");
 }
 
 }  // namespace
@@ -1456,11 +315,11 @@ bool tc_tower_supported(const NetDims& d) {
 }
 
 void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2, bool fast) {
+  (void)fast;  // see tower_tc.cuh: both precision modes run the three fp16 passes
   tower_configure_device();
   Impl* I = new Impl;
   t.impl = I;
   I->d = d; I->n_max = n_max; I->ea = act_scale_log2;
-  if (const char* bs = getenv("AZ_TC_BK")) { if (atoi(bs) == 32) I->bk = 32; }  // experiments: 32 = SWIZZLE_64B, deeper ring
   if (const char* ps = getenv("AZ_TC_PASSES")) { int v = atoi(ps); if (v >= 1 && v <= 3) I->passes = v; }  // experiments only
   // layout choice by padded-row overhead (rows computed per real board point)
   const int S_flat = (d.H + 1) * (d.W + 1), S_ps = d.H * (d.W + 1), tps = (S_ps + BM - 1) / BM;
@@ -1475,60 +334,11 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
   I->xin_hi = alloc_h((size_t)I->rows_alloc * 64); I->xin_lo = alloc_h((size_t)I->rows_alloc * 64);
   for (int i = 0; i < 2; i++) { I->x_hi[i] = alloc_h((size_t)I->rows_alloc * d.K); I->x_lo[i] = alloc_h((size_t)I->rows_alloc * d.K); }
   if (I->mode3d) {
-    I->mIn_hi = make_map3d(I->xin_hi, n_max, I->S, 64, I->bk); I->mIn_lo = make_map3d(I->xin_lo, n_max, I->S, 64, I->bk);
-    for (int i = 0; i < 2; i++) { I->mX_hi[i] = make_map3d(I->x_hi[i], n_max, I->S, d.K, I->bk); I->mX_lo[i] = make_map3d(I->x_lo[i], n_max, I->S, d.K, I->bk); }
+    I->mIn_hi = make_map3d(I->xin_hi, n_max, I->S, 64); I->mIn_lo = make_map3d(I->xin_lo, n_max, I->S, 64);
+    for (int i = 0; i < 2; i++) { I->mX_hi[i] = make_map3d(I->x_hi[i], n_max, I->S, d.K); I->mX_lo[i] = make_map3d(I->x_lo[i], n_max, I->S, d.K); }
   } else {
-    I->mIn_hi = make_map(I->xin_hi, I->rows_alloc, 64, BM, I->bk); I->mIn_lo = make_map(I->xin_lo, I->rows_alloc, 64, BM, I->bk);
-    for (int i = 0; i < 2; i++) { I->mX_hi[i] = make_map(I->x_hi[i], I->rows_alloc, d.K, BM, I->bk); I->mX_lo[i] = make_map(I->x_lo[i], I->rows_alloc, d.K, BM, I->bk); }
-  }
-  {
-    // CTA-pair kernel for the fused layers (N tile 256, K block 64): as many clusters as can be co-resident
-    const char* e2 = getenv("AZ_TC_2CTA");
-    const bool want = e2 ? e2[0] != '0' : true;  // AZ_TC_2CTA=0: the single-CTA kernel (A/B experiments)
-    if (want && I->bk == 64 && 2 * d.K >= 256) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(I->num_sms & ~1); cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem_bytes2();
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      int nc = 0;
-      CUDA_CHECK(cudaOccupancyMaxActiveClusters(&nc, k_conv3x3_tc2, &cfg));
-      I->pair_clusters = std::min(nc, I->num_sms / 2);
-    }
-  }
-  // fused layers: hi*hi on kind::f16 + the two correction passes on kind::f8f6f4 (2 tensor passes per MAC instead of 3).
-  // Default = the halo kernel; AZ_TC_FP8=0: three fp16 passes (k_conv3x3_tc2), =1: per-tap FP8 kernel (A/B checks).
-  I->halo = d.W + 2;
-  I->hrows = (BM + 2 * I->halo + 15) & ~15;
-  const bool pair_ok = I->pair_clusters > 0 && 2 * d.K >= 256, halo_ok = pair_ok && I->hrows <= F8H_MAX_HROWS;
-  const int fp8_best = pair_ok ? (halo_ok ? 2 : 1) : 0;
-  I->fp8 = fast ? fp8_best : 0;
-  if (const char* f8 = getenv("AZ_TC_FP8")) { const int v = atoi(f8); if (v >= 0 && v <= 2) I->fp8 = std::min(v, fp8_best); }  // tests / A-B runs
-  I->halo3 = I->fp8 == 0 && halo_ok;
-  if (const char* h3 = getenv("AZ_TC_HALO")) { if (h3[0] == '0') I->halo3 = false; }  // A/B: per-tap three-pass kernel
-  if (I->halo3)
-    for (int i = 0; i < 2; i++) {
-      if (I->mode3d) { I->mXh_hi[i] = make_map3d(I->x_hi[i], n_max, I->S, d.K, 64, I->hrows); I->mXh_lo[i] = make_map3d(I->x_lo[i], n_max, I->S, d.K, 64, I->hrows); }
-      else { I->mXh_hi[i] = make_map(I->x_hi[i], I->rows_alloc, d.K, I->hrows, 64); I->mXh_lo[i] = make_map(I->x_lo[i], I->rows_alloc, d.K, I->hrows, 64); }
-    }
-  if (I->fp8) {
-    I->pa = 0;   // h8 = e5m2(hi16): the fp16 operand's own scale and range
-    I->q = 11;   // l8 = e5m2(lo * 2^11): |lo| <= 2^-11 |hi|; filters' hi parts (max in [2^13, 2^14)) land at 2^2..2^3 in e4m3
-    for (int i = 0; i < 2; i++) {
-      CUDA_CHECK(cudaMalloc(&I->x_h8[i], (size_t)I->rows_alloc * d.K)); CUDA_CHECK(cudaMemset(I->x_h8[i], 0, (size_t)I->rows_alloc * d.K));
-      CUDA_CHECK(cudaMalloc(&I->x_l8[i], (size_t)I->rows_alloc * d.K)); CUDA_CHECK(cudaMemset(I->x_l8[i], 0, (size_t)I->rows_alloc * d.K));
-      if (I->mode3d) { I->mX_h8[i] = make_map3d_u8(I->x_h8[i], n_max, I->S, d.K); I->mX_l8[i] = make_map3d_u8(I->x_l8[i], n_max, I->S, d.K); }
-      else { I->mX_h8[i] = make_map_u8(I->x_h8[i], I->rows_alloc, d.K, BM); I->mX_l8[i] = make_map_u8(I->x_l8[i], I->rows_alloc, d.K, BM); }
-      if (I->fp8 == 2) {
-        if (I->mode3d) {
-          I->mXh_hi[i] = make_map3d(I->x_hi[i], n_max, I->S, d.K, 64, I->hrows);
-          I->mXh_h8[i] = make_map3d_u8(I->x_h8[i], n_max, I->S, d.K, I->hrows); I->mXh_l8[i] = make_map3d_u8(I->x_l8[i], n_max, I->S, d.K, I->hrows);
-        } else {
-          I->mXh_hi[i] = make_map(I->x_hi[i], I->rows_alloc, d.K, I->hrows, 64);
-          I->mXh_h8[i] = make_map_u8(I->x_h8[i], I->rows_alloc, d.K, I->hrows); I->mXh_l8[i] = make_map_u8(I->x_l8[i], I->rows_alloc, d.K, I->hrows);
-        }
-      }
-    }
+    I->mIn_hi = make_map(I->xin_hi, I->rows_alloc, 64, BM); I->mIn_lo = make_map(I->xin_lo, I->rows_alloc, 64, BM);
+    for (int i = 0; i < 2; i++) { I->mX_hi[i] = make_map(I->x_hi[i], I->rows_alloc, d.K, BM); I->mX_lo[i] = make_map(I->x_lo[i], I->rows_alloc, d.K, BM); }
   }
   // layers: init (single), then SharedLayers fused pairs
   const int K = d.K, HW = d.HW();
@@ -1541,23 +351,10 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
     const size_t ktot = (size_t)9 * L.cin;
     L.w_hi = alloc_h((size_t)L.n_total * ktot); L.w_lo = alloc_h((size_t)L.n_total * ktot);
     CUDA_CHECK(cudaMalloc(&L.aff, (size_t)HW * L.n_total * sizeof(float2)));
-    if (L.pair) {
-      // flat layout: an M tile runs across samples, so a warp's 32 rows start at (row % S) and may wrap: the first 32
-      // positions are repeated after the last one
-      L.aff_rows = I->mode3d ? I->S : I->S + 32;
-      CUDA_CHECK(cudaMalloc(&L.affq, (size_t)L.aff_rows * K * 16));
-      L.mAff = make_map_aff(L.affq, L.aff_rows, (uint64_t)K * 4);
-    }
-    L.mB_hi = make_map(L.w_hi, L.n_total, ktot, L.bn, I->bk); L.mB_lo = make_map(L.w_lo, L.n_total, ktot, L.bn, I->bk);
-    if (L.pair && L.bn == 256) { L.mB2_hi = make_map(L.w_hi, L.n_total, ktot, 128, 64); L.mB2_lo = make_map(L.w_lo, L.n_total, ktot, 128, 64); }
-    if (I->fp8 && L.pair && L.bn == 256) {
-      CUDA_CHECK(cudaMalloc(&L.w_h8, (size_t)L.n_total * ktot)); CUDA_CHECK(cudaMalloc(&L.w_l8, (size_t)L.n_total * ktot));
-      L.mB2_h8 = make_map_u8(L.w_h8, L.n_total, ktot, 128); L.mB2_l8 = make_map_u8(L.w_l8, L.n_total, ktot, 128);
-    }
+    L.mB_hi = make_map(L.w_hi, L.n_total, ktot, L.bn); L.mB_lo = make_map(L.w_lo, L.n_total, ktot, L.bn);
     I->layers.push_back(L);
   }
-  I->small = d.K == 64 && !I->mode3d && I->S <= BM && d.W + 2 <= 16 && (int)I->layers.size() <= SN_MAXL && d.F <= 64 &&
-             128 * 8 * 3 + 3 * HW + d.A1 + d.FC <= SN_SCRATCH / 4;
+  I->small = d.K == 64 && !I->mode3d && I->S <= BM && d.W + 2 <= SN_R0 && (int)I->layers.size() <= SN_MAXL && d.F <= 64;
   if (const char* sn = getenv("AZ_TC_SMALLNET")) { if (sn[0] == '0') I->small = false; }  // A/B: the per-layer kernels
   CUDA_CHECK(cudaDeviceSynchronize());
 }
@@ -1565,11 +362,7 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
 int tc_tower_kernel_kind(const TcTower& t) {
   const Impl* I = (const Impl*)t.impl;
   if (!I) return -1;
-  if (I->small) return 5;
-  if (I->fp8 == 2) return 3;
-  if (I->fp8 == 1) return 2;
-  if (I->halo3) return 4;
-  return I->pair_clusters > 0 && 2 * I->d.K >= 256 ? 1 : 0;
+  return I->small ? 5 : 0;
 }
 
 void tc_tower_free(TcTower& t) {
@@ -1577,8 +370,7 @@ void tc_tower_free(TcTower& t) {
   if (!I) return;
   cudaFree(I->xin_hi); cudaFree(I->xin_lo);
   for (int i = 0; i < 2; i++) { cudaFree(I->x_hi[i]); cudaFree(I->x_lo[i]); }
-  for (Layer& L : I->layers) { cudaFree(L.w_hi); cudaFree(L.w_lo); cudaFree(L.aff); cudaFree(L.affq); cudaFree(L.affs); cudaFree(L.w_h8); cudaFree(L.w_l8); }
-  for (int i = 0; i < 2; i++) { cudaFree(I->x_h8[i]); cudaFree(I->x_l8[i]); }
+  for (Layer& L : I->layers) { cudaFree(L.w_hi); cudaFree(L.w_lo); cudaFree(L.aff); }
   for (cudaEvent_t e : I->ev_pool) cudaEventDestroy(e);
   delete I;
   t.impl = nullptr;
@@ -1607,12 +399,9 @@ void tc_tower_prepare(TcTower& t, const NetLayout& NL, const Snapshot& s, cudaSt
       for (size_t i = 0; i < (size_t)K * ci_real * 9; i++) mx = std::max(mx, std::fabs(f[i]));
     }
     int ew = 0;
-    const bool f8 = I->fp8 && L.pair && L.bn == 256;  // FP8 corrections: hi parts up at [2^13, 2^14) so that the e4m3 copies keep bits
-    if (mx > 0 && std::isfinite(mx)) { int e2; frexpf(mx, &e2); ew = (f8 ? 14 : 7) - e2; }  // mx*2^ew in [64,128)
+    if (mx > 0 && std::isfinite(mx)) { int e2; frexpf(mx, &e2); ew = 7 - e2; }  // mx*2^ew in [64,128)
     const float wscale = ldexpf(1.0f, ew);
     std::vector<__half> whi((size_t)L.n_total * ktot, __float2half_rn(0.0f)), wlo((size_t)L.n_total * ktot, __float2half_rn(0.0f));
-    std::vector<uint8_t> wh8(f8 ? (size_t)L.n_total * ktot : 0, 0), wl8(f8 ? (size_t)L.n_total * ktot : 0, 0);
-    const float inv_q = ldexpf(1.0f, -I->q), inv_pa = ldexpf(1.0f, -I->pa);
     std::vector<float2> aff((size_t)HW * L.n_total);
     const int half_bn = L.pair ? L.bn / 2 : L.bn;
     const float fold = ldexpf(1.0f, -(I->ea + ew)) * inv_sd;
@@ -1628,10 +417,6 @@ void tc_tower_prepare(TcTower& t, const NetLayout& NL, const Snapshot& s, cudaSt
           size_t o = (size_t)row * ktot + (size_t)tap * L.cin + ci;
           whi[o] = hh;
           wlo[o] = __float2half_rn(w - __half2float(hh));
-          if (f8) {
-            wh8[o] = (uint8_t)__nv_cvt_float_to_fp8(__half2float(hh) * inv_q, __NV_SATFINITE, __NV_E4M3);
-            wl8[o] = (uint8_t)__nv_cvt_float_to_fp8((w - __half2float(hh)) * inv_pa, __NV_SATFINITE, __NV_E4M3);
-          }
         }
       const float* g = h.data() + u[br]->gamma + (size_t)ch * HW;
       const float* be = h.data() + u[br]->beta + (size_t)ch * HW;
@@ -1639,46 +424,7 @@ void tc_tower_prepare(TcTower& t, const NetLayout& NL, const Snapshot& s, cudaSt
     }
     CUDA_CHECK(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
-    if (f8) {
-      CUDA_CHECK(cudaMemcpy(L.w_h8, wh8.data(), wh8.size(), cudaMemcpyHostToDevice));
-      CUDA_CHECK(cudaMemcpy(L.w_l8, wl8.data(), wl8.size(), cudaMemcpyHostToDevice));
-    }
     CUDA_CHECK(cudaMemcpy(L.aff, aff.data(), aff.size() * sizeof(float2), cudaMemcpyHostToDevice));
-    if (L.pair) {
-      std::vector<float> q((size_t)L.aff_rows * K * 4, 0.0f);
-      const int Wp = d.W + 1;
-      for (int r = 0; r < L.aff_rows; r++) {
-        const int p = r % I->S, y = p / Wp, x = p - y * Wp;
-        if (y >= d.H || x >= d.W) continue;  // zero-border positions
-        const int hw = y * d.W + x;
-        for (int ch = 0; ch < K; ch++) {
-          float* o = q.data() + ((size_t)r * K + ch) * 4;
-          for (int br = 0; br < 2; br++) {
-            o[2 * br] = h[u[br]->gamma + (size_t)ch * HW + hw] * fold;
-            o[2 * br + 1] = h[u[br]->beta + (size_t)ch * HW + hw];
-          }
-        }
-      }
-      CUDA_CHECK(cudaMemcpy(L.affq, q.data(), q.size() * 4, cudaMemcpyHostToDevice));
-    }
-    if (I->small) {  // k_net_small: rows = the 128 positions of a sample's tile, [row / 32][channel][row % 32]
-      const int per = L.pair ? 4 : 2, Wp = d.W + 1;
-      std::vector<float> q((size_t)128 * 64 * per, 0.0f);
-      for (int r = 0; r < 128 && r < I->S; r++) {
-        const int y = r / Wp, x = r - y * Wp;
-        if (y >= d.H || x >= d.W) continue;
-        const int hw = y * d.W + x;
-        for (int ch = 0; ch < 64; ch++) {
-          float* o = q.data() + (((size_t)(r / 32) * 64 + ch) * 32 + (r % 32)) * per;
-          for (int br = 0; br < (L.pair ? 2 : 1); br++) {  // x 2^ea: relu(A'x + B) * s == relu(sA'x + sB) exactly for a power of two
-            o[2 * br] = ldexpf(h[u[br]->gamma + (size_t)ch * HW + hw] * fold, I->ea);
-            o[2 * br + 1] = ldexpf(h[u[br]->beta + (size_t)ch * HW + hw], I->ea);
-          }
-        }
-      }
-      if (!L.affs) CUDA_CHECK(cudaMalloc(&L.affs, q.size() * 4));
-      CUDA_CHECK(cudaMemcpy(L.affs, q.data(), q.size() * 4, cudaMemcpyHostToDevice));
-    }
   }
   (void)NL;
   t.ready = true;
@@ -1692,56 +438,37 @@ void tc_tower_forward(TcTower& t, const NetLayout& NL, const Snapshot& s, Fp32Sc
   const NetDims& d = I->d;
   const float scale = ldexpf(1.0f, I->ea);
   const size_t f0 = I->profile ? I->ev_get(st) : 0;
-  if (I->small) {  // the whole network of every leaf in one launch
+  int cur = 0;
+  if (I->small) {  // every conv layer of every leaf in one launch; the head kernels read its output from x_hi[0] / x_lo[0]
     SmallMaps maps;
     SmallNetArgs a;
-    a.planes = planes; a.n_dev = n_dev; a.n_max = n_max;
-    a.F = d.F; a.H = d.H; a.W = d.W; a.Wp = d.W + 1; a.S = I->S; a.HW = d.HW(); a.A1 = d.A1; a.FC = d.FC;
-    a.nlayers = (int)I->layers.size(); a.ldp = ldp;
-    a.act_scale = scale; a.inv_scale = 1.0f / scale;
-    a.aff0 = reinterpret_cast<const float2*>(I->layers[0].affs);
+    a.planes = planes; a.n_dev = n_dev; a.n_max = n_max; a.F = d.F; a.H = d.H; a.W = d.W; a.Wp = d.W + 1; a.S = I->S;
+    a.HW = d.HW(); a.nlayers = (int)I->layers.size(); a.guard = I->guard; a.passes = I->passes; a.act_scale = scale;
     for (int l = 0; l < SN_MAXL; l++) {
       const Layer& Lr = I->layers[std::min<size_t>(l, I->layers.size() - 1)];
-      maps.hi[l] = Lr.mB_hi; maps.lo[l] = Lr.mB_lo;
-      a.affq[l] = l > 0 && l < a.nlayers ? Lr.affs : nullptr;
+      maps.hi[l] = Lr.mB_hi; maps.lo[l] = Lr.mB_lo; a.aff[l] = Lr.aff;
     }
-    const SnapUnit& pu = s.units[1 + 2 * d.SharedLayers];
-    const SnapUnit& vu = s.units[2 + 2 * d.SharedLayers];
-    a.wp = s.d + pu.filter; a.gp = s.d + pu.gamma; a.bp = s.d + pu.beta;
-    a.wv = s.d + vu.filter; a.gv = s.d + vu.gamma; a.bv = s.d + vu.beta;
-    a.pW = s.d + s.pW; a.pB = s.d + s.pB; a.vW = s.d + s.vW; a.vB = s.d + s.vB; a.voW = s.d + s.voW; a.voB = s.d + s.voB;
-    a.policy = policy; a.value = value; a.err = err_flag;
-    const int grid = std::max(2, std::min((n_max + 1) & ~1, I->num_sms & ~1));  // CTA pairs; the kernel folds it to ~n / 2 CTAs from the device-side n
+    a.out_hi = I->x_hi[0]; a.out_lo = I->x_lo[0]; a.err = err_flag;
     const size_t e0 = I->profile ? I->ev_get(st) : 0;
-    k_net_small<<<grid, SN_THREADS, smem_bytes_small(), st>>>(maps, a); LAUNCH_CHECK();
-    if (I->profile) { const size_t e1 = I->ev_get(st); I->conv_spans.push_back({e0, e1}); I->fwd_spans.push_back({f0, e1}); }
+    k_net_small<<<std::max(1, std::min(n_max, I->num_sms)), NTHREADS, smem_bytes_small(), st>>>(maps, a); LAUNCH_CHECK();
+    if (I->profile) I->conv_spans.push_back({e0, I->ev_get(st)});
     if (launches) (*launches)++;
-    return;
-  }
+  } else {
   {
     size_t total = (size_t)n_max * d.HW() * 64;
     k_pack_planes<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(planes, n_dev, n_max, d.F, d.H, d.W, 64, I->guard, I->S, scale,
                                                                   I->xin_hi, I->xin_lo); LAUNCH_CHECK();
     if (launches) (*launches)++;
   }
-  int cur = 0;
   dispatch_conv(*I, I->layers[0], I->mIn_hi, I->mIn_lo, I->x_hi[0], I->x_lo[0], n_dev, err_flag, st);
   if (launches) (*launches)++;
-  if (I->fp8) {  // the init conv's output also as e5m2 h8 / l8 for the first fused layer
-    const size_t ne = (size_t)I->rows_alloc * d.K;
-    k_split_fp8<<<(unsigned)((ne + 255) / 256), 256, 0, st>>>(I->x_hi[0], I->x_lo[0], ne, ldexpf(1.0f, I->pa), ldexpf(1.0f, I->q),
-                                                             I->x_h8[0], I->x_l8[0]); LAUNCH_CHECK();
-    if (launches) (*launches)++;
-  }
   for (size_t l = 1; l < I->layers.size(); l++) {
     size_t e0 = I->profile ? I->ev_get(st) : 0;
-    if ((I->fp8 == 2 || I->halo3) && I->layers[l].pair && I->layers[l].bn == 256) launch_conv_pair2_f8h(*I, I->layers[l], cur, cur ^ 1, n_dev, err_flag, st);
-    else if (I->fp8 && I->layers[l].pair && I->layers[l].bn == 256) launch_conv_pair2_f8(*I, I->layers[l], cur, cur ^ 1, n_dev, err_flag, st);
-    else
     dispatch_conv(*I, I->layers[l], I->mX_hi[cur], I->mX_lo[cur], I->x_hi[cur ^ 1], I->x_lo[cur ^ 1], n_dev, err_flag, st);
     if (I->profile) I->conv_spans.push_back({e0, I->ev_get(st)});
     if (launches) (*launches)++;
     cur ^= 1;
+  }
   }
   {
     const SnapUnit& pu = s.units[1 + 2 * d.SharedLayers];

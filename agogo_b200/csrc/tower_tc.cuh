@@ -1,4 +1,4 @@
-// agogo_b200 — tcgen05/TMEM/TMA residual tower (K5) interface.
+// agogo_b200 — wgmma/TMA residual tower (K5) interface.
 #pragma once
 #include "nn.cuh"
 
@@ -9,11 +9,11 @@ struct TcTower {
 // shapes the tensor-core tower handles (K multiple of 64, board fits the padded tiling); smaller
 // nets (tic-tac-toe K=3, Connect-4 K=16) run on the fp32 CUDA-core kernels.
 bool tc_tower_supported(const NetDims& d);
-// fast = AZ_FLAG_FAST_TOWER: the fused layers' two correction passes on the FP8 tensor path (E5M2 x E4M3, ~14.5-bit
-// operands) instead of fp16 — 2 tensor passes per MAC instead of 3; default false = fp32-faithful three fp16 passes
+// fast = AZ_FLAG_FAST_TOWER.  This build has no FP8 correction-pass kernel: both values run the fp32-faithful three
+// fp16 passes, so the flag never lowers precision
 void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2, bool fast);
-// 0: single-CTA kernel, 1: CTA-pair per-tap 3 x fp16, 2: CTA-pair per-tap FP8 corrections, 3: halo FP8 corrections,
-// 4: halo 3 x fp16, 5: the whole small net in one kernel (k_net_small) — which kernel runs the fused layers (bench labels)
+// which kernel runs the fused layers (bench labels): 0 = k_conv3x3_tc (wgmma, 3 x fp16), 5 = k_net_small (the whole tower
+// of a K = 64 net in one kernel); -1 = no tensor-core tower
 int tc_tower_kernel_kind(const TcTower& t);
 void tc_tower_free(TcTower& t);
 // split/scale/reorder the snapshot's filters and BN affines into the tensor-core operand layout
@@ -26,7 +26,7 @@ void tc_tower_forward(TcTower& t, const NetLayout& L, const Snapshot& s, Fp32Scr
                       const int* n_dev, int n_max, float* policy, int ldp, float* value, int* err_flag, cudaStream_t st,
                       unsigned long long* launches);
 
-// K7: the 3x3 convolutions of the training pass (forward, backward-data, backward-filter) on tcgen05 (train_tc.cu)
+// K7: the 3x3 convolutions of the training pass (forward, backward-data, backward-filter) on wgmma (train_tc.cu)
 struct TcGemm { void* impl = nullptr; };
 enum {
   TC_OPERAND_PACK = 0,           // absmax -> exponent, split into fp16 hi/lo into the slot

@@ -319,10 +319,11 @@ inline unsigned nblk(size_t n, int t = 256) { return (unsigned)((n + t - 1) / t)
 }  // namespace
 
 // how many position slices the fp32 backward-filter kernel of a unit is launched with (1 = write dW directly)
+// (sized for H100's 132 SMs: a layer with fewer blocks than SMs is sliced to about two blocks per SM)
 static int dw_slices(const UnitH& u, int P) {
   const int blocks = ((u.Ci * u.k * u.k + TT - 1) / TT) * ((u.Co + TT - 1) / TT);
-  if (blocks >= 148) return 1;
-  return std::max(1, std::min({(296 + blocks - 1) / blocks, 64, (P + 255) / 256}));
+  if (blocks >= 132) return 1;
+  return std::max(1, std::min({(264 + blocks - 1) / blocks, 64, (P + 255) / 256}));
 }
 
 struct TrainImpl {
@@ -338,7 +339,7 @@ struct TrainImpl {
   float* wflip = nullptr;  // mirrored/transposed filter of the unit being back-propagated
   float* dwpart = nullptr; // position-sliced partial filter gradients of the few-output layers
   size_t dwpart_n = 0;
-  TcGemm tc;               // 3x3 forward / backward-data convs on tcgen05 (K in {64,128,256}); impl == nullptr -> fp32 tiled
+  TcGemm tc;               // 3x3 forward / backward-data convs on wgmma (K in {64,128,256}); impl == nullptr -> fp32 tiled
   std::vector<void*> allocs;
   float* alloc(size_t n) {
     float* p;
@@ -617,6 +618,6 @@ void train_allreduce_sgd_p2p(float* const* peer_grads, float* const* peer_params
 
 void train_sgd(TrainWS& ws, const NetLayout& L, float* P, float lr, float gscale, cudaStream_t st, unsigned long long* launches) {
   TrainImpl* T = (TrainImpl*)ws.impl;
-  k_sgd<<<(unsigned)std::min<size_t>((L.total / 4 + 255) / 256 + 1, 148 * 16), 256, 0, st>>>(P, T->grads, lr, gscale, L.total); LAUNCH_CHECK();
+  k_sgd<<<(unsigned)std::min<size_t>((L.total / 4 + 255) / 256 + 1, 132 * 16), 256, 0, st>>>(P, T->grads, lr, gscale, L.total); LAUNCH_CHECK();
   if (launches) (*launches)++;
 }

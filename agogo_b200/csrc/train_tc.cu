@@ -1,4 +1,4 @@
-// agogo_b200 — K7 on tensor cores: the 3x3 convolutions of dual.Train (meta.go:16-54) as tcgen05 GEMMs (sm_100a only).
+// agogo_b200 — K7 on tensor cores: the 3x3 convolutions of dual.Train (meta.go:16-54) as wgmma GEMMs (sm_90a).
 // Forward and backward-data run through the tower's kernel (tc_common.cuh) in raw mode; both are the shifted-operand
 // contraction
 //   out[p, n] = sum_tap sum_k A[p + shift(tap), k] * Bm[n, tap*C + k]
@@ -25,42 +25,28 @@ template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_dw_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
         const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, DwArgs a) {
-  constexpr int BK = 64;
   constexpr int A_TILE_BYTES = BM * BK * 2;
-  constexpr int STAGES = num_stages(BN, BK);
-  constexpr int STAGE_BYTES = stage_bytes(BN, BK);
+  constexpr int STAGES = num_stages(BN);
+  constexpr int STAGE_BYTES = stage_bytes(BN);
   constexpr int B_TILE_BYTES = BN * BK * 2;
-  constexpr int TMEM_COLS = 2 * BN >= 512 ? 512 : (2 * BN >= 256 ? 256 : 128);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bars = smem_base + STAGES * STAGE_BYTES;
-  uint32_t* tmem_ptr_smem = (uint32_t*)(smem_al + STAGES * STAGE_BYTES + 128);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int i) { return bars + 8u * (2 * STAGES + i); };
-  auto tempty_bar = [&](int i) { return bars + 8u * (2 * STAGES + 2 + i); };
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-    for (int i = 0; i < 2; i++) { mbar_init(tfull_bar(i), 1); mbar_init(tempty_bar(i), 4); }
+    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMER_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   const int total_items = 9 * a.co_tiles * a.ci_tiles * a.splits;
   auto decode = [&](int item, int& tap, int& mt, int& nt, int& sp) {
     sp = item % a.splits; item /= a.splits;
     nt = item % a.ci_tiles; item /= a.ci_tiles;
     mt = item % a.co_tiles; tap = item / a.co_tiles;
   };
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     if (lane == 0) {
       uint32_t it = 0;
       for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
@@ -84,71 +70,36 @@ k_dw_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUte
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BM, BN) | (1u << 16);  // B operand MN-major
-      uint32_t it = 0, tcount = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x, tcount++) {
-        const int acc = tcount & 1;
-        const uint32_t aph = (tcount >> 1) & 1;
-        mbar_wait(tempty_bar(acc), aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
-        for (int kb = 0; kb < a.kb_per_split; kb++, it++) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-          const uint32_t sa = smem_base + s * STAGE_BYTES;
-          const uint64_t dAh = make_desc_sw<BK>(sa), dAl = make_desc_sw<BK>(sa + A_TILE_BYTES);
-          const uint64_t dBh = make_desc_mn_sw128(sa + 2 * A_TILE_BYTES, 8192), dBl = make_desc_mn_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, 8192);
-#pragma unroll
-          for (int ks = 0; ks < BK / 16; ks++) {
-            const uint64_t adv = (uint64_t)(ks * 32 >> 4);          // A: 16 fp16 along K inside the swizzle atom
-            const uint64_t advb = (uint64_t)(ks * 16 * 128 >> 4);   // B: 16 K-rows of 128 B
-            umma_f16(d_tmem, dAh + adv, dBh + advb, idesc, (kb | ks) ? 1u : 0u);
-            if (a.passes >= 2) umma_f16(d_tmem, dAh + adv, dBl + advb, idesc, 1u);
-            if (a.passes >= 3) umma_f16(d_tmem, dAl + adv, dBh + advb, idesc, 1u);
-          }
-          umma_commit(empty_bar(s));
-        }
-        umma_commit(tfull_bar(acc));
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    uint32_t tcount = 0;
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x, tcount++) {
-      int tap, mt, nt, sp;
-      decode(item, tap, mt, nt, sp);
-      const int acc = tcount & 1;
-      const uint32_t aph = (tcount >> 1) & 1;
-      mbar_wait(tfull_bar(acc), aph);
-      tc_fence_after();
-      const int co = mt * BM + quad * 32 + lane;
-      const uint32_t t_row = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN;
-      float* o = a.partial + ((size_t)(sp * 9 + tap) * a.Co + co) * a.Ci + nt * BN;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t ra[32];
-        tmem_ld32(t_row + c0, ra);
-        tmem_ld_wait();
-        if (co < a.Co) {
-#pragma unroll
-          for (int q = 0; q < 8; q++)
-            reinterpret_cast<float4*>(o + c0)[q] = make_float4(__uint_as_float(ra[4 * q]), __uint_as_float(ra[4 * q + 1]),
-                                                               __uint_as_float(ra[4 * q + 2]), __uint_as_float(ra[4 * q + 3]));
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(acc));
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
+  const int wg = warp >> 2;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+  float acc[BN / 2];
+  uint32_t it = 0;
+  for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+    int tap, mt, nt, sp;
+    decode(item, tap, mt, nt, sp);
+    for (int kb = 0; kb < a.kb_per_split; kb++, it++) {
+      const int s = it % STAGES;
+      const uint32_t ph = (it / STAGES) & 1;
+      mbar_wait(full_bar(s), ph);
+      __syncwarp();
+      const uint32_t sa = smem_base + s * STAGE_BYTES;
+      // B operand MN-major: 16 K-rows of 128 B per k16 step
+      mma_kblock<BN, 1>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
+                        make_desc_mn_sw128(sa + 2 * A_TILE_BYTES, 8192), make_desc_mn_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, 8192),
+                        16 * 128 >> 4, kb == 0, a.passes);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s));
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int co = mt * BM + row0 + 8 * h;
+      if (co >= a.Co) continue;
+      float* o = a.partial + ((size_t)(sp * 9 + tap) * a.Co + co) * a.Ci + nt * BN + col0;
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
   }
 }
 // dW[co][ci][tap] = 2^-(ea+eb) * sum_split partial[split][tap][co][ci]
@@ -266,12 +217,12 @@ __global__ void k_prep_filter(const float* __restrict__ w, int Co, int Ci, int c
 
 // dynamic shared memory opt-in of the instantiations this file launches (per function, per device)
 void train_configure_device() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<256, false, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256, 64)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<128, false, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128, 64)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<64, false, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64, 64)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256, 64)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128, 64)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64, 64)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64)));
 }
 
 }  // namespace
@@ -386,8 +337,8 @@ void tc_gemm_conv(TcGemm& g, const float* x, int Cin, const float* filter, int f
   }
   const int bn = std::min(256, Cout);
   // tensor maps over the (re-used) operand buffers for this shape
-  CUtensorMap mAh = make_map(sl.hi, I->rows_alloc, cpad, BM, 64), mAl = make_map(sl.lo, I->rows_alloc, cpad, BM, 64);
-  CUtensorMap mBh = make_map(I->w_hi, Cout, (uint64_t)9 * cpad, bn, 64), mBl = make_map(I->w_lo, Cout, (uint64_t)9 * cpad, bn, 64);
+  CUtensorMap mAh = make_map(sl.hi, I->rows_alloc, cpad, BM), mAl = make_map(sl.lo, I->rows_alloc, cpad, BM);
+  CUtensorMap mBh = make_map(I->w_hi, Cout, (uint64_t)9 * cpad, bn), mBl = make_map(I->w_lo, Cout, (uint64_t)9 * cpad, bn);
   ConvArgs a;
   a.n_dev = I->dB; a.n_max = I->B; a.S = I->S; a.Wp = d.W + 1; a.H = d.H; a.W = d.W; a.guard = I->guard; a.mode3d = 0; a.tps = 1;
   a.cin = cpad; a.n_total = Cout; a.cout = Cout; a.aff = nullptr; a.out_hi = nullptr; a.out_lo = nullptr; a.act_scale = 1.0f;
@@ -395,11 +346,11 @@ void tc_gemm_conv(TcGemm& g, const float* x, int Cin, const float* filter, int f
   const int max_tiles = ((I->B * I->S + BM - 1) / BM) * (Cout / bn);
   const int grid = std::min(I->num_sms, max_tiles);
   auto launch = [&](auto kern, int BNv) {
-    kern<<<grid, NTHREADS, smem_bytes(BNv, 64), st>>>(mAh, mAl, mBh, mBl, mBh, a); LAUNCH_CHECK();
+    kern<<<grid, NTHREADS, smem_bytes(BNv), st>>>(mAh, mAl, mBh, mBl, a); LAUNCH_CHECK();
   };
-  if (bn == 256) launch(k_conv3x3_tc<256, false, 64>, 256);
-  else if (bn == 128) launch(k_conv3x3_tc<128, false, 64>, 128);
-  else launch(k_conv3x3_tc<64, false, 64>, 64);
+  if (bn == 256) launch(k_conv3x3_tc<256, false>, 256);
+  else if (bn == 128) launch(k_conv3x3_tc<128, false>, 128);
+  else launch(k_conv3x3_tc<64, false>, 64);
   k_unpack_nchw<<<dim3((HW + 31) / 32, (Cout + 31) / 32, I->B), 256, 0, st>>>(I->raw, I->B, Cout, d.H, d.W, Cout, I->guard, I->S, out, accumulate ? 1 : 0); LAUNCH_CHECK();
   if (launches) *launches += nl + 4;
 }
@@ -419,15 +370,15 @@ void tc_gemm_dw(TcGemm& g, const float* x, const float* dz, float* dW, int x_sta
   absmax_exp(dz, n, exp_dz, st);
   k_pack_cmajor<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dz, I->B, C, d.H, d.W, I->ld, I->guard, I->S, exp_dz, I->t_hi, I->t_lo); LAUNCH_CHECK();
   const int bn = std::min(256, C);
-  CUtensorMap mAh = make_map(I->t_hi, I->crow, I->ld, BM, 64), mAl = make_map(I->t_lo, I->crow, I->ld, BM, 64);
-  CUtensorMap mBh = make_map(sx.hi, I->rows_alloc, C, 64, 64), mBl = make_map(sx.lo, I->rows_alloc, C, 64, 64);
+  CUtensorMap mAh = make_map(I->t_hi, I->crow, I->ld, BM), mAl = make_map(I->t_lo, I->crow, I->ld, BM);
+  CUtensorMap mBh = make_map(sx.hi, I->rows_alloc, C, 64), mBl = make_map(sx.lo, I->rows_alloc, C, 64);
   DwArgs a;
   a.co_tiles = (C + BM - 1) / BM; a.ci_tiles = C / bn; a.splits = I->splits; a.kb_per_split = I->kb_per_split;
   a.guard = I->guard; a.Wp = d.W + 1; a.Co = C; a.Ci = C; a.partial = I->partial; a.passes = 3;
   const int items = 9 * a.co_tiles * a.ci_tiles * a.splits;
   const int grid = std::min(I->num_sms, items);
   auto launch = [&](auto kern, int BNv) {
-    kern<<<grid, NTHREADS, smem_bytes(BNv, 64), st>>>(mAh, mAl, mBh, mBl, a); LAUNCH_CHECK();
+    kern<<<grid, NTHREADS, smem_bytes(BNv), st>>>(mAh, mAl, mBh, mBl, a); LAUNCH_CHECK();
   };
   if (bn == 256) launch(k_dw_tc<256>, 256);
   else if (bn == 128) launch(k_dw_tc<128>, 128);

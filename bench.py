@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — self-play throughput of the B200 engine on BASELINE.json's headline config.
+"""bench.py — self-play throughput of the engine on one H100 per rank, on BASELINE.json's headline config.
 
     python bench.py --gpus N --steps K --warmup W          (N>1: launched by torch.distributed.run)
     python bench.py --impl reference --gpus N --steps K --warmup W
+    python bench.py ... --dump-outputs DIR   (also writes the timed path's results as DIR/<name>.npy)
 
 Workload (config.workload = "C3"): 19x19 Go (wq), 1024 concurrent games per GPU, 800 sims/move,
 20-block x 256 dual net (F=18, FC=512, A'=362, DefaultConf batch 256), two random-init nets (agents A
@@ -50,21 +51,12 @@ def flops_per_eval(w):
 
 KERNELS = {
     # az_profile kernel_kind -> (label, tensor passes per algorithmic MAC, precision line)
-    0: ("k_conv3x3_tc<BN,true,64> (fused residual-block conv, one CTA per 128 x BN tile, fp16 hi/lo 3-pass tcgen05)", 3.0,
-        "fp32 semantics on fp16 tensor cores: hi/lo operand split, 3 tcgen05 passes, fp32 TMEM accumulate"),
-    1: ("k_conv3x3_tc2 (fused residual-block conv, CTA pair / cta_group::2, per-tap tiles, fp16 hi/lo 3-pass tcgen05)", 3.0,
-        "fp32 semantics on fp16 tensor cores: hi/lo operand split, 3 tcgen05 passes, fp32 TMEM accumulate"),
-    2: ("k_conv3x3_tc2_f8 (CTA pair, per-tap tiles, hi*hi kind::f16 + E5M2 x E4M3 correction passes kind::f8f6f4)", 2.0,
-        "AZ_FLAG_FAST_TOWER: fp16 main pass + two FP8 correction passes (~14.5-bit operands), fp32 TMEM accumulate"),
-    3: ("k_conv3x3_tc2_halo<true> (CTA pair, activation halo tile + 9 row-shifted descriptor views, hi*hi kind::f16 + "
-        "E5M2 x E4M3 correction passes kind::f8f6f4)", 2.0,
-        "AZ_FLAG_FAST_TOWER: fp16 main pass + two FP8 correction passes (~14.5-bit operands), fp32 TMEM accumulate"),
-    4: ("k_conv3x3_tc2_halo<false> (CTA pair, activation halo tile + 9 row-shifted descriptor views, fp16 hi/lo 3-pass "
-        "tcgen05)", 3.0,
-        "fp32 semantics on fp16 tensor cores: hi/lo operand split, 3 tcgen05 passes, fp32 TMEM accumulate"),
-    5: ("k_net_small (whole 6 x 64 network of a leaf in one CTA: activations resident in shared memory, nine row-shifted "
-        "descriptor views per layer, filters streamed by TMA, fp16 hi/lo 3-pass tcgen05, heads fused)", 3.0,
-        "fp32 semantics on fp16 tensor cores: hi/lo operand split, 3 tcgen05 passes, fp32 TMEM accumulate"),
+    0: ("k_conv3x3_tc<BN,true> (fused residual-block conv, one CTA per 128 x BN tile, two wgmma warpgroups, fp16 hi/lo "
+        "3-pass)", 3.0,
+        "fp32 semantics on fp16 tensor cores: hi/lo operand split, 3 wgmma passes, fp32 register accumulate"),
+    5: ("k_net_small (whole 64-channel tower of a leaf in one CTA: activations resident in shared memory, nine row-shifted "
+        "descriptor views per layer, filters streamed by TMA, fp16 hi/lo 3-pass wgmma)", 3.0,
+        "fp32 semantics on fp16 tensor cores: hi/lo operand split, 3 wgmma passes, fp32 register accumulate"),
 }
 
 
@@ -77,7 +69,7 @@ def make_desc(w, n_games, device, seed, sims=None, batch=None, flags=0):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -116,7 +108,8 @@ def load_peaks():
             p = json.load(f)
         return p, "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA's H100 SXM data sheet (700 W card), dense; not a measured rate
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data-sheet"
 
 
 def oracle_lib():
@@ -190,9 +183,11 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the dual.Train / gradient all-reduce block")
-    ap.add_argument("--no-fast", action="store_true", help="skip the AZ_FLAG_FAST_TOWER arm")
     ap.add_argument("--fast-tower", action="store_true", help="run the main arm with AZ_FLAG_FAST_TOWER (experiments)")
     ap.add_argument("--cpu-steps", type=int, default=24)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's results (root statistics of a seeded sample of games' search trees after "
+                         "the last timed wave, the net's outputs on the fixed probe positions) as DIR/<name>.npy")
     args = ap.parse_args()
     w = dict(WORKLOADS[args.workload])
     if args.games:
@@ -207,7 +202,7 @@ def main():
               "games_per_gpu": w["n_games"], "sims_per_move": w["sims"],
               "parallelism": "games sharded across %d GPU(s), no collective on the self-play path" % world,
               "step": "one MCTS wave = n_games simulations (select -> batched dual-net eval -> expand/backup)",
-              "l2": "inputs larger than L2: activations ~%d MB per conv layer per agent vs 126 MB L2" %
+              "l2": "inputs larger than L2: activations ~%d MB per conv layer per agent vs 50 MB L2 (H100)" %
                     (w["n_games"] // 2 * (w["size"] + 1) ** 2 * w["k"] * 4 * 2 // 2 ** 20),
               "flops_per_eval": fpe}
 
@@ -250,9 +245,6 @@ def main():
     probe = probe_planes(w, 32)
     main_arm = selfplay_arm(ctx, flags=K.FLAG_FAST_TOWER if args.fast_tower else 0, do_e2e=not args.no_e2e, probe=probe,
                             do_train=not args.no_train)
-    fast_arm = None
-    if not args.no_fast and not args.fast_tower and world == 1:
-        fast_arm = selfplay_arm(ctx, flags=K.FLAG_FAST_TOWER, do_e2e=False, probe=probe, do_train=False, steps=min(args.steps, 60))
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
@@ -282,14 +274,15 @@ def main():
     tree = {"counted_bytes_per_sim": tree_bytes / max(sims, 1), "select_children_per_sim": cnt["select_children"] / max(sims, 1),
             "levels_per_sim": cnt["select_levels"] / max(sims, 1), "nodes_created_per_eval": cnt["created"] / max(evals, 1),
             "null_results": cnt["null_results"],
-            "note": "k_select + k_expand_backup take ~0.14 ms of a wave (profiles/r01_summary.md): latency-bound pointer chase, "
-                    "not bandwidth-bound"}
+            "note": "k_select + k_expand_backup: latency-bound pointer chase, not bandwidth-bound"}
     value = main_arm["value"]
     kind = main_arm["prof"].get("kernel_kind", -1)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ctx["collect"], main_arm["probe_out"])
     line = {"metric": "mcts_sims_per_sec", "value": value, "unit": "sims/s", "n_gpus": world, "steps": args.steps,
             "warmup": warmup, "ms_per_step": 1e3 * main_arm["dt_max"] / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "f32",
-            "precision": KERNELS.get(kind, KERNELS[1])[2] + "; parity vs the fp32 oracle: tests/test_gpu_engine.py::"
+            "precision": KERNELS.get(kind, KERNELS[0])[2] + "; parity vs the fp32 oracle: tests/test_gpu_engine.py::"
                          "test_tc_tower_full_depth_c3 (1e-4 on policy and value)",
             "data": "synthetic", "config": config, "moves_per_sec": value / (w["sims"] + 1),
             "evals_per_sec": main_arm["tot_evals"] / main_arm["dt_max"],
@@ -300,18 +293,6 @@ def main():
                       + (" (wave graph replayed; per-launch events in a second region, see roofline.region)" if main_arm.get("roof_arm") else "")}
     if main_arm.get("train") is not None:
         line["train"] = main_arm["train"]
-    if fast_arm is not None:
-        rf = roofline_of(fast_arm, w, peaks, peak_src)
-        dp = float(np.abs(fast_arm["probe_out"][0] - main_arm["probe_out"][0]).max())
-        dv = float(np.abs(fast_arm["probe_out"][1] - main_arm["probe_out"][1]).max())
-        line["fast_tower"] = {"flag": "AZ_FLAG_FAST_TOWER (opt-in)", "value": fast_arm["value"], "unit": "sims/s",
-                              "steps": fast_arm["steps"], "ms_per_step": 1e3 * fast_arm["dt_max"] / fast_arm["steps"],
-                              "roofline": rf, "clocks": fast_arm["clocks"],
-                              "max_abs_dpolicy_vs_default": dp, "max_abs_dvalue_vs_default": dv,
-                              "probe": "%d synthetic 19x19 positions through both precision modes of THIS run's nets" % len(probe),
-                              "note": "FP8 correction passes (E5M2 x E4M3): ~14.5-bit operands; within 1.3e-5 of the fp32 oracle "
-                                      "on well-conditioned nets, up to 1.4e-4 on the reference's random init (gain > 1 per "
-                                      "layer) — outside the 1e-4 bar, hence not the default"}
     print(json.dumps(line))
     return 0
 
@@ -330,13 +311,43 @@ def probe_planes(w, n):
     return x.reshape(n, -1)
 
 
+DUMP_GAMES = 32  # games whose trees --dump-outputs samples (fixed seed: the same games on every run with the same arguments)
+
+
+def root_children(e, n_games):
+    """Root and first-level rows of both agents' trees of a seeded sample of games, as the last timed wave left them:
+    float64 [rows, 9] = {game, tree, depth, move, visits, W, P, expanded, n_children} (tree_dump's columns, W and P as
+    the float32 values their bits hold)."""
+    games = np.sort(np.random.default_rng(20240).choice(n_games, size=min(DUMP_GAMES, n_games), replace=False))
+    out = []
+    for g in games:
+        for t in (0, 1):
+            rows = e.tree_dump(int(g), t)
+            rows = rows[rows[:, 0] <= 1]
+            r = np.empty((len(rows), 9), np.float64)
+            r[:, 0], r[:, 1] = g, t
+            r[:, 2:5] = rows[:, 0:3]
+            r[:, 5] = rows[:, 3].view(np.float32)
+            r[:, 6] = rows[:, 4].view(np.float32)
+            r[:, 7:9] = rows[:, 5:7]
+            out.append(r)
+    return np.concatenate(out) if out else np.zeros((0, 9))
+
+
+def dump_outputs(d, root_rows, probe_out):
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "root_children.npy"), root_rows)
+    np.save(os.path.join(d, "probe_policy.npy"), np.asarray(probe_out[0], np.float32))
+    np.save(os.path.join(d, "probe_value.npy"), np.asarray(probe_out[1], np.float32))
+
+
 def roofline_of(arm, w, peaks, peak_src):
     prof, evals = arm["prof"], arm["cnt"]["evals"]
     hw = w["size"] ** 2
     kind = prof.get("kernel_kind", -1)
-    label, passes, _ = KERNELS.get(kind, KERNELS[1])
-    if w["k"] < 128 and kind in (0, 1):
-        label = "k_conv3x3_tc<%d,true,64> (fused residual-block conv, one CTA per 128 x %d tile, fp16 hi/lo 3-pass tcgen05)" % (2 * w["k"], 2 * w["k"])
+    label, passes, _ = KERNELS.get(kind, KERNELS[0])
+    if w["k"] < 128 and kind == 0:
+        label = label.replace("<BN,true>", "<%d,true>" % (2 * w["k"])).replace("128 x BN", "128 x %d" % (2 * w["k"]))
     # dominant kernel: the fused 3x3 conv of one residual block (both branches, C -> 2C), one launch per block per agent.
     # Algorithmic FLOPs of all its launches in the timed region: every evaluated leaf passes through `blocks` of them
     conv_flops = 2 * 9 * w["k"] * (2 * w["k"]) * hw * evals * w["blocks"]
@@ -344,18 +355,10 @@ def roofline_of(arm, w, peaks, peak_src):
     achieved = conv_flops / conv_s / 1e12 if conv_s > 0 else None
     peak = peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops"))
     traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "conv_traffic.json")  # per-kernel dram bytes per launch from committed ncu --set full captures
-    if os.path.exists(tp):
-        try:
-            ent = json.load(open(tp)).get("%s/%d" % (arm["workload"], kind))
-            if ent:
-                traffic, traffic_src = ent["dram_bytes_per_launch"], ent["source"]
-        except Exception:
-            pass
     pad = {19: 384.0 / 361.0, 9: 100.0 / 81.0}.get(w["size"], 1.0)
     return {"bound": "tensor", "kernel": label, "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
             "frac": (achieved / peak) if achieved else None,
-            "peak_source": "%s bf16 dense, sustained (kernel timed inside a long step)" % peak_src,
+            "peak_source": "%s bf16 dense" % peak_src,
             "traffic": traffic, "traffic_source": traffic_src, "launches_timed": prof["conv_launches"],
             "avg_launch_ms": prof["conv_ms"] / max(prof["conv_launches"], 1),
             "algorithmic_flops_per_launch": conv_flops / max(prof["conv_launches"], 1),
@@ -421,6 +424,8 @@ def selfplay_arm(ctx, flags, do_e2e, probe, do_train, steps=None):
     e.profile(True)
     two_regions = e.profile(False)["kernel_kind"] == 5
     prof, clocks, cnt = timed_region(2 if two_regions else 1)
+    if args.dump_outputs and ctx.get("collect") is None:  # exactly `steps` waves in, whether or not a re-measure follows
+        ctx["collect"] = root_children(e, n_games)
     bad = {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"}
     if bad & set(clocks.get("reasons", [])) and world == 1:  # rejected: re-measure once (timing rules)
         prof, clocks2, cnt = timed_region(2 if two_regions else 1)
@@ -502,8 +507,8 @@ def train_block(ctx, e, w):
             gbs = nbytes / (ms / 1e3) / 1e9
             res.update({"k8_kernel": "k_allreduce_sgd_p2p (reduce-scatter + SGD + all-gather over NVLink peer memory, one kernel)",
                         "k8_ms": ms, "nvlink_bytes_per_rank_per_direction": nbytes, "gbs_per_direction": gbs,
-                        "peak_gbs_per_direction": 770.0, "frac": gbs / 770.0,
-                        "peak_source": "measured peer copy, /opt/skills/guides/B200_PROFILING.md"})
+                        "peak_gbs_per_direction": 450.0, "frac": gbs / 450.0,
+                        "peak_source": "H100 SXM data sheet: NVLink 900 GB/s bidirectional (not measured)"})
         rng = np.random.default_rng(5 + rank)
         X = rng.choice([0.0, 1.0, -1.0], size=(B, 18 * hw)).astype(np.float32)
         Pi = np.zeros((B, hw + 1), np.float32)

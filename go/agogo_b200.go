@@ -1,4 +1,4 @@
-// Package b200 is the cgo shim that puts the B200 engine (include/agogo_b200.h) under gorgonia/agogo's
+// Package b200 is the cgo shim that puts the H100 engine (include/agogo_b200.h) under gorgonia/agogo's
 // Go API.  UNCOMPILED in this repository's image (no Go toolchain); kept as the binding a maintainer
 // would add next to agent.go / arena.go / agogo.go.  No Go pointer is retained by C after a call, and no Go-allocated
 // struct containing Go pointers is passed to C (az_state's arrays are C.malloc copies).  backend_b200.go puts the

@@ -1,6 +1,6 @@
 // +build b200
 
-// Drop-in bodies for the hot-path methods of package agogo on top of the B200 engine (package b200, agogo_b200.go).
+// Drop-in bodies for the hot-path methods of package agogo on top of the H100 engine (package b200, agogo_b200.go).
 // UNCOMPILED here (no Go toolchain in this image).  A maintainer adds this file to the root package and tags the
 // reference's own bodies `// +build !b200`: agent.go (Search, SwitchToInference, useDummy, resetStats), arena.go (Play,
 // newB), agogo.go (New, SelfPlay, Learn, Save, Load).  Every signature below is the reference's, so callers — cmd/*,

@@ -1,5 +1,5 @@
 /*
- * agogo_b200.h — C ABI of the B200-native AlphaZero self-play engine that slots under
+ * agogo_b200.h — C ABI of the H100-native AlphaZero self-play engine that slots under
  * gorgonia/agogo's Go API (AZ / Agent / Arena, game.State, mcts.Config, dual.Config).
  *
  * The reference has no FFI boundary (one Go process, Go interfaces only); every entry point
@@ -13,7 +13,7 @@
  * engine returns AZ_ERR_PANIC and the Go shim re-panics.
  *
  * Two libraries export exactly these symbols:
- *   agogo_b200/libagogo_b200.so   the product: hand-written sm_100a CUDA, fails loudly without a GPU
+ *   agogo_b200/libagogo_b200.so   the product: hand-written sm_90a CUDA, fails loudly without a GPU
  *   oracle/libazoracle.so         TEST INFRASTRUCTURE: CPU restatement of the reference algorithm
  */
 #ifndef AGOGO_B200_H
@@ -96,13 +96,10 @@ typedef struct az_dual_config {
 } az_dual_config;
 
 #define AZ_FLAG_SHARED_TREE 1u /* one MCTS searched by both colours (mcts/example_test.go:74-156) */
-#define AZ_FLAG_FP32_TOWER 2u  /* force the fp32 CUDA-core tower (validation kernel) instead of tcgen05 */
-/* Precision policy of the tcgen05 tower.  Default: fp32-faithful — fp16 hi/lo operand split, three tensor passes per MAC,
- * policy/value within 1e-4 of the fp32 forward on every net measured (incl. the reference's own random init, whose
- * per-layer gain > 1 leaves a 1.5x margin).  AZ_FLAG_FAST_TOWER: the two correction passes run on the FP8 tensor path
- * (E5M2 activations x E4M3 filters, ~14.5-bit effective operands, two tensor passes per MAC): +26 % simulations/s, outputs
- * within 1.3e-5 on well-conditioned nets but up to 1.4e-4 on the reference's untamed init — outside the 1e-4 bar, hence
- * opt-in (DESIGN.md section 4). */
+#define AZ_FLAG_FP32_TOWER 2u  /* force the fp32 CUDA-core tower (validation kernel) instead of the tensor cores */
+/* Precision policy of the tensor-core tower: fp32-faithful — fp16 hi/lo operand split, three tensor passes per MAC,
+ * policy/value within 1e-4 of the fp32 forward (DESIGN.md section 4).  AZ_FLAG_FAST_TOWER is accepted for a faster,
+ * less precise tower; this build has no such kernel and runs the three passes for it too. */
 #define AZ_FLAG_FAST_TOWER 4u
 /* wq only — OUR completion of the reference's unfinished Go rules (SURVEY section 8f row 4), off by default (the default
  * keeps wq.Game exactly as written: occupied points "legal", no ko, the row-0 flood-fill Score).  With the flag:
@@ -123,7 +120,7 @@ typedef struct az_engine_desc {
   int32_t device;   /* CUDA device ordinal */
   uint32_t flags;
   uint64_t seed;    /* replaces the reference's time.Now() seeds (arena.go:61, tree.go:84) */
-  int32_t act_scale_log2;     /* tcgen05 tower: activations are stored as fp16 hi/lo of x*2^this; 0 = default (-2: |x| up to 2.6e5
+  int32_t act_scale_log2;     /* tensor-core tower: activations are stored as fp16 hi/lo of x*2^this; 0 = default (-2: |x| up to 2.6e5
                                * before AZ_ERR_PANIC "activation overflow"; outputs are insensitive to it between -5 and 5) */
   int32_t max_nodes_per_tree; /* 0 = derive from sims and action space */
 } az_engine_desc;
@@ -274,12 +271,11 @@ int az_counters_reset(az_engine* e);
  * measurement, enable=0 stops; out (may be NULL) receives {conv_ms_total, conv_launches,
  * forward_ms_total, forward_calls, region_ms, kernel_kind, 0...} accumulated since the last enable=1; region_ms is the
  * device time between the enable=1 and the enable=0 call on the engine's stream; kernel_kind names the kernel that runs
- * the fused layers (0 single-CTA, 1 CTA-pair per-tap 3 x fp16, 2 per-tap FP8 corrections, 3 halo FP8 corrections,
- * 4 halo 3 x fp16, 5 k_net_small; -1 fp32 tower).  enable=2 times the region only (region_ms): no per-launch events, so
+ * the fused layers (0 k_conv3x3_tc, wgmma, three fp16 passes; 5 k_net_small; -1 fp32 tower).  enable=2 times the region only (region_ms): no per-launch events, so
  * the captured wave graph keeps running — what a launch-bound small-net workload should be timed with. */
 int az_profile(az_engine* e, int32_t enable, double out[8]);
 
-const char* az_build_info(void); /* "agogo_b200 <ver> sm_100a ..." or "oracle ..." */
+const char* az_build_info(void); /* "agogo_b200 <ver> sm_90a ..." or "oracle ..." */
 
 #ifdef __cplusplus
 }

@@ -10,7 +10,7 @@ ORACLE_SO = os.path.join(ROOT, "oracle", "libazoracle.so")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def _build_oracle():

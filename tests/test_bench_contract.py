@@ -44,9 +44,9 @@ def test_roofline_arithmetic():
     import bench
     w = bench.WORKLOADS["C3"]
     assert bench.flops_per_eval(w) == 17065507816      # SURVEY section 8d: 17.07 GFLOP per 19x19 20x256 evaluation
-    arm = dict(prof=dict(conv_ms=800.0, conv_launches=1000.0, kernel_kind=4), cnt=dict(evals=25600), dt=1.0, workload="C3")
+    arm = dict(prof=dict(conv_ms=800.0, conv_launches=1000.0, kernel_kind=0), cnt=dict(evals=25600), dt=1.0, workload="C3")
     r = bench.roofline_of(arm, w, {"bf16_tflops_sustained": 1465.8}, "measured")
     per_launch = 2 * 9 * 256 * 512 * 361 * 25600 * 20 / 1000.0
     assert abs(r["algorithmic_flops_per_launch"] - per_launch) < 1 and abs(r["achieved"] - per_launch * 1000 / 0.8 / 1e12) < 1e-6
     assert abs(r["frac"] - r["achieved"] / 1465.8) < 1e-12 and r["tensor_passes_per_mac"] == 3.0
-    assert "halo" in r["kernel"] and r["bound"] == "tensor" and r["unit"] == "TFLOP/s"
+    assert "wgmma" in r["kernel"] and "<BN,true>" in r["kernel"] and r["bound"] == "tensor" and r["unit"] == "TFLOP/s"

@@ -32,7 +32,7 @@ def product():
 def test_product_exports_every_declared_symbol(product):
     for name in _declared():
         assert hasattr(product.dll, name), name
-    assert "sm_100a" in product.build_info()
+    assert "sm_90a" in product.build_info()
 
 
 def test_oracle_exports_every_declared_symbol(oracle):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """dual.Train step (K7) timing: forward (BN train mode) + loss + backward + SGD on one batch.  3x3 layers with
-K in {64,128,256} run forward / backward-data / backward-filter on the tcgen05 kernels (AZ_TRAIN_TC=0 forces the fp32
+K in {64,128,256} run forward / backward-data / backward-filter on the wgmma kernels (AZ_TRAIN_TC=0 forces the fp32
 CUDA-core kernels of train.cu, which every other layer uses).  Prints one JSON line per shape with the algorithmic FLOPs (3 x forward) and the achieved rate."""
 import json
 import os

@@ -1,8 +1,7 @@
 #!/usr/bin/env python
 """Two (or more) ranks, a small c4 net, a few data-parallel az_train steps through the fused peer-memory all-reduce + SGD
-kernel — the workload the sanitizer runs wrap (profiles/r02_sanitizer.md):
-    python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 --no-python \
-        compute-sanitizer --tool memcheck python tools/k8_small.py"""
+kernel:
+    python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 tools/k8_small.py"""
 import os
 import sys
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Feasibility arithmetic for DESIGN.md §10: error of a Winograd F(2x2,3x3) formulation of one tower layer when its 16
-element-wise GEMMs run as fp16 hi/lo 3-pass products with fp32 accumulation (what tcgen05 kind::f16 gives), against the
+element-wise GEMMs run as fp16 hi/lo 3-pass products with fp32 accumulation (what the fp16 tensor cores give), against the
 direct 9-tap form with the same split — both measured against an fp64 convolution.  CPU only (numpy), one layer,
 C = 256, 19x19, a few boards; activations are ReLU outputs, filters GlorotU like the reference's init."""
 import numpy as np
