@@ -7,6 +7,8 @@
 // stages (full/empty mbarriers); warps 0-7 are two consumer warpgroups, each owning 64 of the tile's 128 M rows and
 // issuing wgmma.mma_async (m64 x BN x k16, both operands from shared memory, fp32 accumulators in registers), then
 // running the epilogue straight from its registers while the producer already fills the next tile's stages.
+// The number of tensor passes is a template parameter: a K block is one wgmma group with nothing between its wgmmas,
+// so ptxas emits one warpgroup.arrive per block instead of fencing every wgmma.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -27,6 +29,7 @@ constexpr int BK = 64;         // K block per pipeline stage: 64 fp16 = 128-byte
 constexpr int NTHREADS = 288;  // warps 0-7: two consumer warpgroups; warp 8: TMA producer
 constexpr int PRODUCER_WARP = 8;
 constexpr int CONSUMER_WARPS = 8;
+constexpr int TC_PASSES = 3;   // hi*hi + hi*lo + lo*hi (fp32-faithful); 2 drops lo*hi, 1 is hi*hi only (diagnostics)
 // H100: 227 KB of dynamic shared memory per block, less alignment slack and the barriers
 constexpr int SMEM_RING_BUDGET = 227 * 1024 - 2048;
 __host__ __device__ constexpr int stage_bytes(int BN) { return 2 * BM * BK * 2 + 2 * BN * BK * 2; }
@@ -203,33 +206,33 @@ struct ConvArgs {
   __half* out_lo;
   float act_scale;    // 2^ea
   int* err;
-  int passes;         // 3: hi*hi + hi*lo + lo*hi (fp32-faithful, default); 2: drops lo*hi; 1: hi*hi only
   // raw mode (training, K7): no affine / ReLU / split — the epilogue writes acc * 2^-(*exp_a + *exp_b) as fp32
   float* out_raw;     // [(guard + rows)][n_total] or nullptr
   const int* exp_a;   // power-of-two scales of the A and B operands (device: they are data dependent)
   const int* exp_b;
 };
 
-// One K block of the three-pass product for this warpgroup's 64 rows: A rows at a_hi / a_lo, B (BN rows) at b_hi / b_lo.
+// One K block of the PASSES-pass product for this warpgroup's 64 rows: A rows at a_hi / a_lo, B (BN rows) at b_hi / b_lo.
 // a_step / b_step: descriptor start-address advance (16-byte units) per 16-wide K step.
-template <int BN, int TB>
+template <int BN, int TB, int PASSES = TC_PASSES>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t dAh, uint64_t dAl, uint64_t dBh, uint64_t dBl,
-                                           uint32_t b_step, bool first, int passes, uint32_t a_step = 32 >> 4) {
+                                           uint32_t b_step, bool first, uint32_t a_step = 32 >> 4) {
+  static_assert(PASSES >= 1 && PASSES <= 3, "1 to 3 passes");
   wgmma_fence();
 #pragma unroll
   for (int ks = 0; ks < BK / 16; ks++) {
     const uint64_t adv = (uint64_t)ks * a_step;     // A: K-major SWIZZLE_128B: 16 fp16 = 32 B inside the atom
     const uint64_t advb = (uint64_t)ks * b_step;    // B: K-major as A; MN-major 16 K-rows of 128 B
     wgmma_f16<BN, TB>(acc, dAh + adv, dBh + advb, (first && ks == 0) ? 0u : 1u);
-    if (passes >= 2) wgmma_f16<BN, TB>(acc, dAh + adv, dBl + advb, 1u);
-    if (passes >= 3) wgmma_f16<BN, TB>(acc, dAl + adv, dBh + advb, 1u);
+    if constexpr (PASSES >= 2) wgmma_f16<BN, TB>(acc, dAh + adv, dBl + advb, 1u);
+    if constexpr (PASSES >= 3) wgmma_f16<BN, TB>(acc, dAl + adv, dBh + advb, 1u);
   }
   wgmma_commit();
   wgmma_wait_all();
   acc_fence(acc);
 }
 
-template <int BN, bool PAIR>
+template <int BN, bool PAIR, int PASSES = TC_PASSES>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
              const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, ConvArgs a) {
@@ -305,9 +308,9 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
       mbar_wait(full_bar(s), ph);
       __syncwarp();
       const uint32_t sa = smem_base + s * STAGE_BYTES;
-      mma_kblock<BN, 0>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
-                        make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
-                        kb == 0, a.passes);
+      mma_kblock<BN, 0, PASSES>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
+                                make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
+                                kb == 0);
       __syncwarp();
       if (lane == 0) mbar_arrive(empty_bar(s));  // this warp's share of the stage has been read
     }

@@ -107,7 +107,7 @@ struct SmallMaps { CUtensorMap hi[SN_MAXL], lo[SN_MAXL]; };
 struct SmallNetArgs {
   const float* planes;  // [n][F][HW] encoder planes
   const int* n_dev;
-  int n_max, F, H, W, Wp, S, HW, nlayers, guard, passes;
+  int n_max, F, H, W, Wp, S, HW, nlayers, guard;
   float act_scale;
   const float2* aff[SN_MAXL];  // per layer [HW][n_total] {A', B}
   __half *out_hi, *out_lo;     // last layer: [(guard + n*S)][64], the layout k_head_convs_nhwc reads
@@ -131,7 +131,7 @@ __device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int sm
     const uint32_t shift = (uint32_t)(SN_R0 + wg * 64 + (tap / 3 - 1) * a.Wp + (tap % 3 - 1)) * 16;
     const uint32_t sb = ring + st * SN_STAGE;
     mma_kblock<N, 0>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_lo + shift, SN_HR * 16),
-                     make_desc_sw(sb), make_desc_sw(sb + SN_STAGE / 2), 32 >> 4, tap == 0, a.passes, 2 * SN_HR * 16 >> 4);
+                     make_desc_sw(sb), make_desc_sw(sb + SN_STAGE / 2), 32 >> 4, tap == 0, 2 * SN_HR * 16 >> 4);
     __syncwarp();
     if (lane == 0) mbar_arrive(bars + 8u * (SN_NST + st));
   }
@@ -247,13 +247,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
 
 // dynamic shared memory opt-in of every instantiation this file launches, on the current device (the attribute is per
 // function and per device; called from the allocator, which runs with the engine's device current)
-template <int BN, bool PAIR>
+template <int BN, bool PAIR, int PASSES = TC_PASSES>
 void set_conv_attr() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN)));
 }
 void tower_configure_device() {
   set_conv_attr<256, true>(); set_conv_attr<128, true>(); set_conv_attr<256, false>(); set_conv_attr<128, false>();
   set_conv_attr<64, false>();
+  set_conv_attr<256, true, 1>(); set_conv_attr<256, true, 2>(); set_conv_attr<128, true, 1>(); set_conv_attr<128, true, 2>();
   CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small()));
 }
 
@@ -266,7 +267,7 @@ struct Layer {
 };
 struct Impl {
   NetDims d;
-  int n_max, ea, guard, S, rows_alloc, num_sms, passes = 3, mode3d = 0, tps = 1;
+  int n_max, ea, guard, S, rows_alloc, num_sms, passes = TC_PASSES, mode3d = 0, tps = 1;
   bool small = false;  // K = 64, (H+1)(W+1) <= 128: the whole tower of a sample in one kernel (k_net_small)
   __half *xin_hi = nullptr, *xin_lo = nullptr;  // [(guard+rows+guard)][64]
   __half *x_hi[2] = {nullptr, nullptr}, *x_lo[2] = {nullptr, nullptr};  // [(guard+rows+guard)][K]
@@ -284,22 +285,27 @@ struct Impl {
   }
 };
 
-template <int BN, bool PAIR>
+template <int BN, bool PAIR, int PASSES = TC_PASSES>
 void launch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
                  const int* n_dev, int* err, cudaStream_t st) {
   ConvArgs a;
   a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
   a.mode3d = I.mode3d; a.tps = I.tps;
   a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff; a.out_hi = ohi; a.out_lo = olo;
-  a.act_scale = ldexpf(1.0f, I.ea); a.err = err; a.passes = I.passes;
+  a.act_scale = ldexpf(1.0f, I.ea); a.err = err;
   a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
   const int max_tiles = (I.mode3d ? I.n_max * I.tps : (I.n_max * I.S + BM - 1) / BM) * (L.n_total / BN);
   const int grid = std::min(I.num_sms, max_tiles);
-  k_conv3x3_tc<BN, PAIR><<<grid, NTHREADS, smem_bytes(BN), st>>>(ah, al, L.mB_hi, L.mB_lo, a); LAUNCH_CHECK();
+  k_conv3x3_tc<BN, PAIR, PASSES><<<grid, NTHREADS, smem_bytes(BN), st>>>(ah, al, L.mB_hi, L.mB_lo, a); LAUNCH_CHECK();
 }
 void dispatch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
                    const int* n_dev, int* err, cudaStream_t st) {
-  if (L.pair && L.bn == 256) launch_conv<256, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  // AZ_TC_PASSES (diagnostics) selects 1 or 2 passes for the fused layers; the other shapes always run three
+  if (L.pair && L.bn == 256 && I.passes == 1) launch_conv<256, true, 1>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (L.pair && L.bn == 256 && I.passes == 2) launch_conv<256, true, 2>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (L.pair && L.bn == 256) launch_conv<256, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (L.pair && L.bn == 128 && I.passes == 1) launch_conv<128, true, 1>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  else if (L.pair && L.bn == 128 && I.passes == 2) launch_conv<128, true, 2>(I, L, ah, al, ohi, olo, n_dev, err, st);
   else if (L.pair && L.bn == 128) launch_conv<128, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
   else if (!L.pair && L.bn == 256) launch_conv<256, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
   else if (!L.pair && L.bn == 128) launch_conv<128, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
@@ -443,7 +449,7 @@ void tc_tower_forward(TcTower& t, const NetLayout& NL, const Snapshot& s, Fp32Sc
     SmallMaps maps;
     SmallNetArgs a;
     a.planes = planes; a.n_dev = n_dev; a.n_max = n_max; a.F = d.F; a.H = d.H; a.W = d.W; a.Wp = d.W + 1; a.S = I->S;
-    a.HW = d.HW(); a.nlayers = (int)I->layers.size(); a.guard = I->guard; a.passes = I->passes; a.act_scale = scale;
+    a.HW = d.HW(); a.nlayers = (int)I->layers.size(); a.guard = I->guard; a.act_scale = scale;
     for (int l = 0; l < SN_MAXL; l++) {
       const Layer& Lr = I->layers[std::min<size_t>(l, I->layers.size() - 1)];
       maps.hi[l] = Lr.mB_hi; maps.lo[l] = Lr.mB_lo; a.aff[l] = Lr.aff;

@@ -19,7 +19,6 @@ struct DwArgs {
   int co_tiles, ci_tiles, splits, kb_per_split;
   int guard, Wp, Co, Ci;
   float* partial;  // [splits][9][Co][Ci]
-  int passes;
 };
 template <int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
@@ -88,7 +87,7 @@ k_dw_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUte
       // B operand MN-major: 16 K-rows of 128 B per k16 step
       mma_kblock<BN, 1>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
                         make_desc_mn_sw128(sa + 2 * A_TILE_BYTES, 8192), make_desc_mn_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, 8192),
-                        16 * 128 >> 4, kb == 0, a.passes);
+                        16 * 128 >> 4, kb == 0);
       __syncwarp();
       if (lane == 0) mbar_arrive(empty_bar(s));
     }
@@ -342,7 +341,7 @@ void tc_gemm_conv(TcGemm& g, const float* x, int Cin, const float* filter, int f
   ConvArgs a;
   a.n_dev = I->dB; a.n_max = I->B; a.S = I->S; a.Wp = d.W + 1; a.H = d.H; a.W = d.W; a.guard = I->guard; a.mode3d = 0; a.tps = 1;
   a.cin = cpad; a.n_total = Cout; a.cout = Cout; a.aff = nullptr; a.out_hi = nullptr; a.out_lo = nullptr; a.act_scale = 1.0f;
-  a.err = nullptr; a.passes = 3; a.out_raw = I->raw; a.exp_a = sl.exp; a.exp_b = I->exp_b;
+  a.err = nullptr; a.out_raw = I->raw; a.exp_a = sl.exp; a.exp_b = I->exp_b;
   const int max_tiles = ((I->B * I->S + BM - 1) / BM) * (Cout / bn);
   const int grid = std::min(I->num_sms, max_tiles);
   auto launch = [&](auto kern, int BNv) {
@@ -374,7 +373,7 @@ void tc_gemm_dw(TcGemm& g, const float* x, const float* dz, float* dW, int x_sta
   CUtensorMap mBh = make_map(sx.hi, I->rows_alloc, C, 64), mBl = make_map(sx.lo, I->rows_alloc, C, 64);
   DwArgs a;
   a.co_tiles = (C + BM - 1) / BM; a.ci_tiles = C / bn; a.splits = I->splits; a.kb_per_split = I->kb_per_split;
-  a.guard = I->guard; a.Wp = d.W + 1; a.Co = C; a.Ci = C; a.partial = I->partial; a.passes = 3;
+  a.guard = I->guard; a.Wp = d.W + 1; a.Co = C; a.Ci = C; a.partial = I->partial;
   const int items = 9 * a.co_tiles * a.ci_tiles * a.splits;
   const int grid = std::min(I->num_sms, items);
   auto launch = [&](auto kern, int BNv) {
