@@ -343,7 +343,7 @@ int az_engine_create(const az_engine_desc* desc, az_engine** out) {
     fp32_scratch_alloc(e->fp32, nd, E.GS);
     e->use_tc = !(desc->flags & AZ_FLAG_FP32_TOWER) && tc_tower_supported(nd);
     if (e->use_tc)
-      for (int a = 0; a < 2; a++) tc_tower_alloc(e->tc[a], nd, E.GS, desc->act_scale_log2 ? desc->act_scale_log2 : -2, (desc->flags & AZ_FLAG_FAST_TOWER) != 0);
+      for (int a = 0; a < 2; a++) tc_tower_alloc(e->tc[a], nd, E.GS, desc->act_scale_log2 ? desc->act_scale_log2 : -2);
 
     CUDA_CHECK(cudaMallocHost(&e->h_ex_board, (size_t)G * P.plane * 4));
     CUDA_CHECK(cudaMallocHost(&e->h_ex_policy, (size_t)G * (P.A + 1) * 4));
@@ -424,7 +424,7 @@ int az_agent_set_inferer(az_engine* e, int32_t agent, int32_t kind, int32_t dumm
   InfererDev& I = e->E.inf[agent];
   if (kind == AZ_INF_DUAL) {
     snapshot_gather(e->L, e->net_params[agent], e->snap[agent], e->stream);
-    if (e->use_tc) tc_tower_prepare(e->tc[agent], e->L, e->snap[agent], e->stream, &e->launches);
+    if (e->use_tc) tc_tower_prepare(e->tc[agent], e->snap[agent], e->stream);
     CUDA_CHECK(cudaStreamSynchronize(e->stream));
     e->snap_valid[agent] = true;
     I.kind = INF_DUAL; I.L = e->d.nn.action_space;

@@ -36,6 +36,13 @@ __host__ __device__ constexpr int stage_bytes(int BN) { return 2 * BM * BK * 2 +
 __host__ __device__ constexpr int num_stages(int BN) { return SMEM_RING_BUDGET / stage_bytes(BN) > 8 ? 8 : SMEM_RING_BUDGET / stage_bytes(BN); }
 __host__ __device__ constexpr int smem_bytes(int BN) { return num_stages(BN) * stage_bytes(BN) + 1024 + 256; }
 
+// The operand format of every tensor-core pass: v = hi + lo, hi = fp16(v), lo = fp16(v - hi).  Callers scale v by a
+// power of two first so that lo stays a normal fp16.
+__host__ __device__ __forceinline__ void split_hi_lo(float v, __half& hi, __half& lo) {
+  hi = __float2half_rn(v);
+  lo = __float2half_rn(v - __half2float(hi));
+}
+
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -60,6 +67,34 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         : "memory");
   } while (!ok);
 }
+// The stage ring of every kernel here: full[STAGES] then empty[STAGES] mbarriers at `bars`.  Pipeline step `it` uses
+// stage it % STAGES in phase (it / STAGES) & 1.  The producer's lane waits until every consumer warp has released the
+// stage's previous use, then arms full with the bytes its TMA loads will deliver; a consumer warp waits on full and,
+// once its MMAs have read the stage, releases it with one arrival from lane 0.
+template <int STAGES>
+struct MbarRing {
+  uint32_t bars;
+  __device__ __forceinline__ static uint32_t stage(uint32_t it) { return it % STAGES; }
+  __device__ __forceinline__ uint32_t full(uint32_t it) const { return bars + 8u * stage(it); }
+  __device__ __forceinline__ uint32_t empty(uint32_t it) const { return bars + 8u * (STAGES + stage(it)); }
+  __device__ __forceinline__ void init(uint32_t consumer_arrivals) const {  // by thread 0; the caller then __syncthreads
+    if (threadIdx.x != 0) return;
+    for (int s = 0; s < STAGES; s++) { mbar_init(full(s), 1); mbar_init(empty(s), consumer_arrivals); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __device__ __forceinline__ void producer_acquire(uint32_t it, uint32_t bytes) const {
+    mbar_wait(empty(it), ((it / STAGES) & 1) ^ 1);
+    mbar_expect_tx(full(it), bytes);
+  }
+  __device__ __forceinline__ void consumer_wait(uint32_t it) const {
+    mbar_wait(full(it), (it / STAGES) & 1);
+    __syncwarp();
+  }
+  __device__ __forceinline__ void consumer_release(uint32_t it) const {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(empty(it));
+  }
+};
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -232,6 +267,33 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t dAh, u
   acc_fence(acc);
 }
 
+// This consumer thread's place in its warpgroup's m64nNk16 accumulator fragment (warpgroup wg = warp / 4 owns tile rows
+// wg*64 .. wg*64 + 63): acc[4j + 2h + e] = (tile row row0 + 8h, column 8j + col0 + e)
+__device__ __forceinline__ void acc_frag_origin(int warp, int lane, int& row0, int& col0) {
+  row0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+  col0 = 2 * (lane & 3);
+}
+
+// Output value of a fused layer at output column 8j + col0 + e of fragment row half h, before the hi/lo split: BN affine
+// and ReLU, for a fused pair (PAIR) plus the second branch's, whose weight rows sit N/2 columns further in the tile, then
+// the activation scale.  aff points at the tile's affine row of this position, offset by col0.
+template <int N, bool PAIR>
+__device__ __forceinline__ float fused_value(const float2* aff, const float (&acc)[N / 2], int j, int h, int e, float act_scale) {
+  constexpr int OUTC = PAIR ? N / 2 : N;
+  const float2 fa = __ldg(aff + 8 * j + e);
+  float v = fmaxf(fmaf(fa.x, acc[4 * j + 2 * h + e], fa.y), 0.0f);
+  if (PAIR) {
+    const float2 fb = __ldg(aff + N / 2 + 8 * j + e);
+    v += fmaxf(fmaf(fb.x, acc[4 * (j + OUTC / 8) + 2 * h + e], fb.y), 0.0f);
+  }
+  return v * act_scale;
+}
+
+// M tiles of a convolution over n samples: whole tiles per sample in the per-sample layout, else over the flat rows
+__host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n) {
+  return a.mode3d ? n * a.tps : (n * a.S + BM - 1) / BM;
+}
+
 template <int BN, bool PAIR, int PASSES = TC_PASSES>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
@@ -243,20 +305,14 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
   constexpr int OUTC = PAIR ? BN / 2 : BN;  // output channels per N tile
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + STAGES * STAGE_BYTES;  // full[S], empty[S]
+  const MbarRing<STAGES> ring{smem_base + STAGES * STAGE_BYTES};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  auto full_bar = [&](int s) { return bars + 8u * s; };
-  auto empty_bar = [&](int s) { return bars + 8u * (STAGES + s); };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMER_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  ring.init(CONSUMER_WARPS);
   __syncthreads();
 
   const int n = min(*a.n_dev, a.n_max);
   const int rows = n * a.S;
-  const int m_tiles = a.mode3d ? n * a.tps : (rows + BM - 1) / BM;
+  const int m_tiles = conv_m_tiles(a, n);
   const int n_tiles = a.n_total / BN;
   const int total_tiles = m_tiles * n_tiles;
   const int kc_per_tap = a.cin / BK;
@@ -270,24 +326,21 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
         const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
         const int m0 = mt * BM, n0 = nt * BN;
         for (int kb = 0; kb < kblocks; kb++, it++) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
+          ring.producer_acquire(it, STAGE_BYTES);
           const int tap = kb / kc_per_tap, kc = kb - tap * kc_per_tap;
           const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-          const uint32_t sa = smem_base + s * STAGE_BYTES;
-          mbar_expect_tx(full_bar(s), STAGE_BYTES);
+          const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES, bar = ring.full(it);
           if (a.mode3d) {
             const int b = mt / a.tps, p0 = (mt - b * a.tps) * BM + dy * a.Wp + dx;  // may be <0 / >=S: zero fill
-            tma_load_3d(sa, &tmA_hi, full_bar(s), kc * BK, p0, b);
-            tma_load_3d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), kc * BK, p0, b);
+            tma_load_3d(sa, &tmA_hi, bar, kc * BK, p0, b);
+            tma_load_3d(sa + A_TILE_BYTES, &tmA_lo, bar, kc * BK, p0, b);
           } else {
             const int arow = a.guard + m0 + dy * a.Wp + dx;
-            tma_load_2d(sa, &tmA_hi, full_bar(s), kc * BK, arow);
-            tma_load_2d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), kc * BK, arow);
+            tma_load_2d(sa, &tmA_hi, bar, kc * BK, arow);
+            tma_load_2d(sa + A_TILE_BYTES, &tmA_lo, bar, kc * BK, arow);
           }
-          tma_load_2d(sa + 2 * A_TILE_BYTES, &tmB_hi, full_bar(s), tap * a.cin + kc * BK, n0);
-          tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, full_bar(s), tap * a.cin + kc * BK, n0);
+          tma_load_2d(sa + 2 * A_TILE_BYTES, &tmB_hi, bar, tap * a.cin + kc * BK, n0);
+          tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, bar, tap * a.cin + kc * BK, n0);
         }
       }
     }
@@ -295,24 +348,20 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
   }
   // ===== consumer warpgroups 0 and 1: rows wg*64 .. wg*64+63 of the tile =====
   const int wg = warp >> 2;
-  // accumulator fragment of m64nBNk16: acc[4j + 2h + e] = (row 16*(warp&3) + lane/4 + 8h, column 8j + 2*(lane&3) + e)
-  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+  int row0, col0;
+  acc_frag_origin(warp, lane, row0, col0);
   float acc[BN / 2];
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
     const int m0 = mt * BM, n0 = nt * BN;
     for (int kb = 0; kb < kblocks; kb++, it++) {
-      const int s = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      mbar_wait(full_bar(s), ph);
-      __syncwarp();
-      const uint32_t sa = smem_base + s * STAGE_BYTES;
+      ring.consumer_wait(it);
+      const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES;
       mma_kblock<BN, 0, PASSES>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
                                 make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
                                 kb == 0);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(s));  // this warp's share of the stage has been read
+      ring.consumer_release(it);
     }
     // ===== epilogue from registers =====
     bool overflow = false;
@@ -351,18 +400,8 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
         __half hv[2], lv[2];
 #pragma unroll
         for (int e = 0; e < 2; e++) {
-          const float2 fa = __ldg(aff + 8 * j + e);
-          float v = fmaxf(fmaf(fa.x, acc[4 * j + 2 * h + e], fa.y), 0.0f);
-          if (PAIR) {
-            const float2 fb = __ldg(aff + BN / 2 + 8 * j + e);
-            v += fmaxf(fmaf(fb.x, acc[4 * (j + OUTC / 8) + 2 * h + e], fb.y), 0.0f);
-          }
-          v *= a.act_scale;
-          const __half hh = __float2half_rn(v);
-          const float hf = __half2float(hh);
-          overflow |= !(fabsf(hf) <= 65504.0f);
-          hv[e] = hh;
-          lv[e] = __float2half_rn(v - hf);
+          split_hi_lo(fused_value<BN, PAIR>(aff, acc, j, h, e, a.act_scale), hv[e], lv[e]);
+          overflow |= !(fabsf(__half2float(hv[e])) <= 65504.0f);
         }
         *reinterpret_cast<__half2*>(ohi + 8 * j) = __halves2half2(hv[0], hv[1]);
         *reinterpret_cast<__half2*>(olo + 8 * j) = __halves2half2(lv[0], lv[1]);
@@ -370,6 +409,19 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
     }
     if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
   }
+}
+
+// dynamic shared memory opt-in of one instantiation on the current device (the attribute is per function and per device)
+template <int BN, bool PAIR, int PASSES = TC_PASSES>
+void set_conv_attr() {
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN)));
+}
+// persistent grid: one CTA per SM, or one per tile when the largest batch has fewer
+template <int BN, bool PAIR, int PASSES = TC_PASSES>
+void launch_conv(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl, const ConvArgs& a,
+                 int num_sms, cudaStream_t st) {
+  const int grid = std::min(num_sms, conv_m_tiles(a, a.n_max) * (a.n_total / BN));
+  k_conv3x3_tc<BN, PAIR, PASSES><<<grid, NTHREADS, smem_bytes(BN), st>>>(ah, al, bh, bl, a); LAUNCH_CHECK();
 }
 
 // ---------------------------------------------------------------------------------------------

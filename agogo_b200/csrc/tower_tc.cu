@@ -23,6 +23,12 @@
 
 namespace {
 
+// the first layer's input at (sample b, channel c, board point hw) before the hi/lo split: the scaled encoder plane, zero
+// off the board and in the channels padded beyond F (k_pack_planes and k_net_small write the same operand)
+__device__ __forceinline__ float plane_input(const float* planes, int F, int HW, int b, int c, int hw, bool on_board, float scale) {
+  return on_board && c < F ? planes[((size_t)b * F + c) * HW + hw] * scale : 0.0f;
+}
+
 // fp32 NCHW planes -> zero-bordered NHWC fp16 hi/lo (channels padded to cpad)
 __global__ void k_pack_planes(const float* __restrict__ planes, const int* __restrict__ n_dev, int n_max, int F, int H,
                               int W, int cpad, int guard, int S, float scale, __half* hi, __half* lo) {
@@ -34,11 +40,11 @@ __global__ void k_pack_planes(const float* __restrict__ planes, const int* __res
   const int hw = (int)((idx / cpad) % HW);
   const int b = (int)(idx / ((size_t)cpad * HW));
   const int y = hw / W, x = hw - y * W;
-  float v = c < F ? planes[((size_t)b * F + c) * HW + hw] * scale : 0.0f;
-  __half h = __float2half_rn(v);
+  __half h, l;
+  split_hi_lo(plane_input(planes, F, HW, b, c, hw, true, scale), h, l);
   const size_t o = ((size_t)guard + (size_t)b * S + y * Wp + x) * cpad + c;
   hi[o] = h;
-  lo[o] = __float2half_rn(v - __half2float(h));
+  lo[o] = l;
 }
 // The two 1x1 head convs (K->2 policy, K->1 value; dual.go:70,85) + BN-test affine + ReLU straight
 // from the tower's NHWC hi/lo output: one warp per board point, lanes split the channels
@@ -116,24 +122,22 @@ struct SmallNetArgs {
 
 // one layer of one sample: 9 taps of the filter ring into acc, then the epilogue into smem (or global for the last layer)
 template <int N>
-__device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int smp, uint32_t act, uint32_t ring, uint32_t bars,
-                                            uint32_t& it, int in, bool& overflow) {
+__device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int smp, uint32_t act, uint32_t stages,
+                                            const MbarRing<SN_NST>& ring, uint32_t& it, int in, bool& overflow) {
   constexpr bool PAIR = N == 128;
   constexpr int OUTC = PAIR ? N / 2 : N;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+  int row0, col0;
+  acc_frag_origin(warp, lane, row0, col0);
   const uint32_t in_hi = act + (2 * in) * SN_PLANE, in_lo = in_hi + SN_PLANE;
   float acc[N / 2];
   for (int tap = 0; tap < 9; tap++, it++) {
-    const int st = it % SN_NST;
-    mbar_wait(bars + 8u * st, (it / SN_NST) & 1);
-    __syncwarp();
+    ring.consumer_wait(it);
     const uint32_t shift = (uint32_t)(SN_R0 + wg * 64 + (tap / 3 - 1) * a.Wp + (tap % 3 - 1)) * 16;
-    const uint32_t sb = ring + st * SN_STAGE;
+    const uint32_t sb = stages + ring.stage(it) * SN_STAGE;
     mma_kblock<N, 0>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_lo + shift, SN_HR * 16),
                      make_desc_sw(sb), make_desc_sw(sb + SN_STAGE / 2), 32 >> 4, tap == 0, 2 * SN_HR * 16 >> 4);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bars + 8u * (SN_NST + st));
+    ring.consumer_release(it);
   }
   const bool last = l == a.nlayers - 1;
   const uint32_t out_hi = act + (2 * (in ^ 1)) * SN_PLANE, out_lo = out_hi + SN_PLANE;
@@ -151,21 +155,8 @@ __device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int sm
       __half hv[2], lv[2];
 #pragma unroll
       for (int e = 0; e < 2; e++) {
-        float v = 0.0f;
-        if (valid) {
-          const float2 fa = __ldg(aff + 8 * j + e);
-          v = fmaxf(fmaf(fa.x, acc[4 * j + 2 * h + e], fa.y), 0.0f);
-          if (PAIR) {
-            const float2 fb = __ldg(aff + N / 2 + 8 * j + e);
-            v += fmaxf(fmaf(fb.x, acc[4 * (j + OUTC / 8) + 2 * h + e], fb.y), 0.0f);
-          }
-          v *= a.act_scale;
-        }
-        const __half hh = __float2half_rn(v);
-        const float hf = __half2float(hh);
-        overflow |= !(fabsf(hf) <= 65504.0f);
-        hv[e] = hh;
-        lv[e] = __float2half_rn(v - hf);
+        split_hi_lo(valid ? fused_value<N, PAIR>(aff, acc, j, h, e, a.act_scale) : 0.0f, hv[e], lv[e]);
+        overflow |= !(fabsf(__half2float(hv[e])) <= 65504.0f);
       }
       const int c = 8 * j + col0;
       if (last) {
@@ -188,15 +179,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t act = base;                     // 4 planes: buffer b hi at 2b, lo at 2b + 1
-  const uint32_t ring = base + 4 * SN_PLANE;      // filter stages (1024-aligned: SN_PLANE is a multiple of 1024)
-  const uint32_t bars = ring + SN_NST * SN_STAGE; // full[NST], empty[NST]
+  const uint32_t act = base;                       // 4 planes: buffer b hi at 2b, lo at 2b + 1
+  const uint32_t stages = base + 4 * SN_PLANE;      // filter stages (1024-aligned: SN_PLANE is a multiple of 1024)
+  const MbarRing<SN_NST> ring{stages + SN_NST * SN_STAGE};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int i = threadIdx.x; i < 4 * SN_PLANE / 16; i += blockDim.x) reinterpret_cast<uint4*>(base_ptr)[i] = make_uint4(0, 0, 0, 0);
-  if (threadIdx.x == 0) {
-    for (int st = 0; st < SN_NST; st++) { mbar_init(bars + 8u * st, 1); mbar_init(bars + 8u * (SN_NST + st), CONSUMER_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  ring.init(CONSUMER_WARPS);
   proxy_fence();  // the zeroed halo rows are read by wgmma
   __syncthreads();
   const int n = min(*a.n_dev, a.n_max);
@@ -207,12 +195,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
         for (int l = 0; l < a.nlayers; l++) {
           const uint32_t bytes = 2u * (l == 0 ? 64 : 128) * BK * 2;
           for (int tap = 0; tap < 9; tap++, it++) {
-            const int st = it % SN_NST;
-            mbar_wait(bars + 8u * (SN_NST + st), ((it / SN_NST) & 1) ^ 1);
-            const uint32_t sb = ring + st * SN_STAGE;
-            mbar_expect_tx(bars + 8u * st, bytes);
-            tma_load_2d(sb, &maps.hi[l], bars + 8u * st, tap * BK, 0);
-            tma_load_2d(sb + SN_STAGE / 2, &maps.lo[l], bars + 8u * st, tap * BK, 0);
+            ring.producer_acquire(it, bytes);
+            const uint32_t sb = stages + ring.stage(it) * SN_STAGE;
+            tma_load_2d(sb, &maps.hi[l], ring.full(it), tap * BK, 0);
+            tma_load_2d(sb + SN_STAGE / 2, &maps.lo[l], ring.full(it), tap * BK, 0);
           }
         }
     }
@@ -226,18 +212,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
     for (int i = tid; i < 128 * 64; i += 256) {
       const int p = i >> 6, c = i & 63;
       const int y = p / a.Wp, x = p - y * a.Wp;
-      float v = 0.0f;
-      if (p < a.S && y < a.H && x < a.W && c < a.F) v = a.planes[((size_t)smp * a.F + c) * a.HW + y * a.W + x] * a.act_scale;
-      const __half h = __float2half_rn(v);
+      const float v = plane_input(a.planes, a.F, a.HW, smp, c, y * a.W + x, p < a.S && y < a.H && x < a.W, a.act_scale);
       const uint32_t o = (uint32_t)(c >> 3) * (SN_HR * 16) + (uint32_t)(SN_R0 + p) * 16 + (uint32_t)(c & 7) * 2;
-      *reinterpret_cast<__half*>(base_ptr + o) = h;
-      *reinterpret_cast<__half*>(base_ptr + SN_PLANE + o) = __float2half_rn(v - __half2float(h));
+      split_hi_lo(v, *reinterpret_cast<__half*>(base_ptr + o), *reinterpret_cast<__half*>(base_ptr + SN_PLANE + o));
     }
     proxy_fence();
     consumer_sync();
     for (int l = 0; l < a.nlayers; l++) {
-      if (l == 0) small_layer<64>(a, l, smp, act, ring, bars, it, 0, overflow);
-      else small_layer<128>(a, l, smp, act, ring, bars, it, l & 1, overflow);
+      if (l == 0) small_layer<64>(a, l, smp, act, stages, ring, it, 0, overflow);
+      else small_layer<128>(a, l, smp, act, stages, ring, it, l & 1, overflow);
       proxy_fence();   // this layer's generic smem writes are read by the next layer's wgmma (async proxy)
       consumer_sync(); // and every warp's MMAs on the buffer the next layer overwrites have completed
     }
@@ -245,12 +228,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
   if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
 }
 
-// dynamic shared memory opt-in of every instantiation this file launches, on the current device (the attribute is per
-// function and per device; called from the allocator, which runs with the engine's device current)
-template <int BN, bool PAIR, int PASSES = TC_PASSES>
-void set_conv_attr() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN)));
-}
+// dynamic shared memory opt-in of every instantiation this file launches, on the current device (called from the
+// allocator, which runs with the engine's device current)
 void tower_configure_device() {
   set_conv_attr<256, true>(); set_conv_attr<128, true>(); set_conv_attr<256, false>(); set_conv_attr<128, false>();
   set_conv_attr<64, false>();
@@ -285,31 +264,27 @@ struct Impl {
   }
 };
 
-template <int BN, bool PAIR, int PASSES = TC_PASSES>
-void launch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
-                 const int* n_dev, int* err, cudaStream_t st) {
+// AZ_TC_PASSES (diagnostics) selects 1 or 2 passes for the fused layers; the other shapes always run three
+template <int BN>
+void launch_fused(int passes, const CUtensorMap& ah, const CUtensorMap& al, const Layer& L, const ConvArgs& a, int num_sms,
+                  cudaStream_t st) {
+  if (passes == 1) launch_conv<BN, true, 1>(ah, al, L.mB_hi, L.mB_lo, a, num_sms, st);
+  else if (passes == 2) launch_conv<BN, true, 2>(ah, al, L.mB_hi, L.mB_lo, a, num_sms, st);
+  else launch_conv<BN, true>(ah, al, L.mB_hi, L.mB_lo, a, num_sms, st);
+}
+void dispatch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
+                   const int* n_dev, int* err, cudaStream_t st) {
   ConvArgs a;
   a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
   a.mode3d = I.mode3d; a.tps = I.tps;
   a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff; a.out_hi = ohi; a.out_lo = olo;
   a.act_scale = ldexpf(1.0f, I.ea); a.err = err;
   a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
-  const int max_tiles = (I.mode3d ? I.n_max * I.tps : (I.n_max * I.S + BM - 1) / BM) * (L.n_total / BN);
-  const int grid = std::min(I.num_sms, max_tiles);
-  k_conv3x3_tc<BN, PAIR, PASSES><<<grid, NTHREADS, smem_bytes(BN), st>>>(ah, al, L.mB_hi, L.mB_lo, a); LAUNCH_CHECK();
-}
-void dispatch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
-                   const int* n_dev, int* err, cudaStream_t st) {
-  // AZ_TC_PASSES (diagnostics) selects 1 or 2 passes for the fused layers; the other shapes always run three
-  if (L.pair && L.bn == 256 && I.passes == 1) launch_conv<256, true, 1>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (L.pair && L.bn == 256 && I.passes == 2) launch_conv<256, true, 2>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (L.pair && L.bn == 256) launch_conv<256, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (L.pair && L.bn == 128 && I.passes == 1) launch_conv<128, true, 1>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (L.pair && L.bn == 128 && I.passes == 2) launch_conv<128, true, 2>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (L.pair && L.bn == 128) launch_conv<128, true>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (!L.pair && L.bn == 256) launch_conv<256, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (!L.pair && L.bn == 128) launch_conv<128, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
-  else if (!L.pair && L.bn == 64) launch_conv<64, false>(I, L, ah, al, ohi, olo, n_dev, err, st);
+  if (L.pair && L.bn == 256) launch_fused<256>(I.passes, ah, al, L, a, I.num_sms, st);
+  else if (L.pair && L.bn == 128) launch_fused<128>(I.passes, ah, al, L, a, I.num_sms, st);
+  else if (!L.pair && L.bn == 256) launch_conv<256, false>(ah, al, L.mB_hi, L.mB_lo, a, I.num_sms, st);
+  else if (!L.pair && L.bn == 128) launch_conv<128, false>(ah, al, L.mB_hi, L.mB_lo, a, I.num_sms, st);
+  else if (!L.pair && L.bn == 64) launch_conv<64, false>(ah, al, L.mB_hi, L.mB_lo, a, I.num_sms, st);
   else throw std::runtime_error("tc tower: unsupported tile");
 }
 
@@ -320,8 +295,7 @@ bool tc_tower_supported(const NetDims& d) {
   return (d.K == 64 || d.K == 128 || d.K == 256) && d.F <= 64 && d.SharedLayers >= 0;
 }
 
-void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2, bool fast) {
-  (void)fast;  // see tower_tc.cuh: both precision modes run the three fp16 passes
+void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2) {
   tower_configure_device();
   Impl* I = new Impl;
   t.impl = I;
@@ -330,7 +304,6 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
   // layout choice by padded-row overhead (rows computed per real board point)
   const int S_flat = (d.H + 1) * (d.W + 1), S_ps = d.H * (d.W + 1), tps = (S_ps + BM - 1) / BM;
   I->mode3d = (tps * BM < S_flat) ? 1 : 0;
-  if (const char* m = getenv("AZ_TC_LAYOUT")) I->mode3d = m[0] == '3';  // experiments: "3" / "2"
   if (I->mode3d) { I->guard = 0; I->S = S_ps; I->tps = tps; I->rows_alloc = n_max * I->S; }
   else { I->guard = ((d.W + 2 + 7) / 8) * 8; I->S = S_flat; I->tps = 1; I->rows_alloc = I->guard + n_max * I->S + I->guard + BM; }
   int dev;
@@ -385,7 +358,7 @@ void tc_tower_free(TcTower& t) {
 // Host-side operand preparation (once per Agent.SwitchToInference): split the fp32 filters into
 // fp16 hi/lo at a per-layer power-of-two scale, reorder rows so that an N tile holds the same
 // output channels of both branches, fold BN-test (x/sqrt(eps)), gamma and the scales into A'.
-void tc_tower_prepare(TcTower& t, const NetLayout& NL, const Snapshot& s, cudaStream_t st, unsigned long long*) {
+void tc_tower_prepare(TcTower& t, const Snapshot& s, cudaStream_t st) {
   Impl* I = (Impl*)t.impl;
   const NetDims& d = I->d;
   const int K = d.K, HW = d.HW();
@@ -418,11 +391,8 @@ void tc_tower_prepare(TcTower& t, const NetLayout& NL, const Snapshot& s, cudaSt
       const float* f = h.data() + u[br]->filter + (size_t)ch * ci_real * 9;
       for (int tap = 0; tap < 9; tap++)
         for (int ci = 0; ci < ci_real; ci++) {
-          float w = f[ci * 9 + tap] * wscale;  // filter[co][ci][ky][kx], tap = ky*3+kx
-          __half hh = __float2half_rn(w);
-          size_t o = (size_t)row * ktot + (size_t)tap * L.cin + ci;
-          whi[o] = hh;
-          wlo[o] = __float2half_rn(w - __half2float(hh));
+          const size_t o = (size_t)row * ktot + (size_t)tap * L.cin + ci;
+          split_hi_lo(f[ci * 9 + tap] * wscale, whi[o], wlo[o]);  // filter[co][ci][ky][kx], tap = ky*3+kx
         }
       const float* g = h.data() + u[br]->gamma + (size_t)ch * HW;
       const float* be = h.data() + u[br]->beta + (size_t)ch * HW;
@@ -432,7 +402,6 @@ void tc_tower_prepare(TcTower& t, const NetLayout& NL, const Snapshot& s, cudaSt
     CUDA_CHECK(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemcpy(L.aff, aff.data(), aff.size() * sizeof(float2), cudaMemcpyHostToDevice));
   }
-  (void)NL;
   t.ready = true;
 }
 

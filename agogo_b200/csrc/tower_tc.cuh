@@ -9,15 +9,13 @@ struct TcTower {
 // shapes the tensor-core tower handles (K multiple of 64, board fits the padded tiling); smaller
 // nets (tic-tac-toe K=3, Connect-4 K=16) run on the fp32 CUDA-core kernels.
 bool tc_tower_supported(const NetDims& d);
-// fast = AZ_FLAG_FAST_TOWER.  This build has no FP8 correction-pass kernel: both values run the fp32-faithful three
-// fp16 passes, so the flag never lowers precision
-void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2, bool fast);
+void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2);
 // which kernel runs the fused layers (bench labels): 0 = k_conv3x3_tc (wgmma, 3 x fp16), 5 = k_net_small (the whole tower
 // of a K = 64 net in one kernel); -1 = no tensor-core tower
 int tc_tower_kernel_kind(const TcTower& t);
 void tc_tower_free(TcTower& t);
 // split/scale/reorder the snapshot's filters and BN affines into the tensor-core operand layout
-void tc_tower_prepare(TcTower& t, const NetLayout& L, const Snapshot& s, cudaStream_t st, unsigned long long* launches);
+void tc_tower_prepare(TcTower& t, const Snapshot& s, cudaStream_t st);
 // event timing of the fused-block conv launches (bench roofline); collect() synchronises the stream
 void tc_tower_profile(TcTower& t, bool enable);
 void tc_tower_profile_collect(TcTower& t, cudaStream_t st, double* conv_ms, double* conv_launches, double* fwd_ms,

@@ -30,14 +30,9 @@ k_dw_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUte
   constexpr int B_TILE_BYTES = BN * BK * 2;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t bars = smem_base + STAGES * STAGE_BYTES;
+  const MbarRing<STAGES> ring{smem_base + STAGES * STAGE_BYTES};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  auto full_bar = [&](int s) { return bars + 8u * s; };
-  auto empty_bar = [&](int s) { return bars + 8u * (STAGES + s); };
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; s++) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMER_WARPS); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
+  ring.init(CONSUMER_WARPS);
   __syncthreads();
   const int total_items = 9 * a.co_tiles * a.ci_tiles * a.splits;
   auto decode = [&](int item, int& tap, int& mt, int& nt, int& sp) {
@@ -53,18 +48,15 @@ k_dw_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUte
         decode(item, tap, mt, nt, sp);
         const int shift = (tap / 3 - 1) * a.Wp + (tap % 3 - 1);
         for (int kb = 0; kb < a.kb_per_split; kb++, it++) {
-          const int s = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          const uint32_t sa = smem_base + s * STAGE_BYTES;
+          ring.producer_acquire(it, STAGE_BYTES);
+          const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES, bar = ring.full(it);
           const int col = a.guard + (sp * a.kb_per_split + kb) * BK;
-          mbar_expect_tx(full_bar(s), STAGE_BYTES);
-          tma_load_2d(sa, &tmA_hi, full_bar(s), col, mt * BM);
-          tma_load_2d(sa + A_TILE_BYTES, &tmA_lo, full_bar(s), col, mt * BM);
+          tma_load_2d(sa, &tmA_hi, bar, col, mt * BM);
+          tma_load_2d(sa + A_TILE_BYTES, &tmA_lo, bar, col, mt * BM);
 #pragma unroll
           for (int j = 0; j < BN / 64; j++) {  // [64 positions][64 channels] boxes, one per 64-wide N group
-            tma_load_2d(sa + 2 * A_TILE_BYTES + j * 8192, &tmB_hi, full_bar(s), nt * BN + j * 64, col + shift);
-            tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES + j * 8192, &tmB_lo, full_bar(s), nt * BN + j * 64, col + shift);
+            tma_load_2d(sa + 2 * A_TILE_BYTES + j * 8192, &tmB_hi, bar, nt * BN + j * 64, col + shift);
+            tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES + j * 8192, &tmB_lo, bar, nt * BN + j * 64, col + shift);
           }
         }
       }
@@ -72,24 +64,21 @@ k_dw_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUte
     return;
   }
   const int wg = warp >> 2;
-  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col0 = 2 * (lane & 3);
+  int row0, col0;
+  acc_frag_origin(warp, lane, row0, col0);
   float acc[BN / 2];
   uint32_t it = 0;
   for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
     int tap, mt, nt, sp;
     decode(item, tap, mt, nt, sp);
     for (int kb = 0; kb < a.kb_per_split; kb++, it++) {
-      const int s = it % STAGES;
-      const uint32_t ph = (it / STAGES) & 1;
-      mbar_wait(full_bar(s), ph);
-      __syncwarp();
-      const uint32_t sa = smem_base + s * STAGE_BYTES;
+      ring.consumer_wait(it);
+      const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES;
       // B operand MN-major: 16 K-rows of 128 B per k16 step
       mma_kblock<BN, 1>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
                         make_desc_mn_sw128(sa + 2 * A_TILE_BYTES, 8192), make_desc_mn_sw128(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, 8192),
                         16 * 128 >> 4, kb == 0);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(s));
+      ring.consumer_release(it);
     }
 #pragma unroll
     for (int h = 0; h < 2; h++) {
@@ -122,11 +111,8 @@ __global__ void k_pack_cmajor(const float* __restrict__ x, int B, int C, int H, 
   if (idx >= (size_t)B * C * HW) return;
   const int hw = (int)(idx % HW), c = (int)((idx / HW) % C), b = (int)(idx / ((size_t)HW * C));
   const int y = hw / W, xx = hw - y * W;
-  const float v = x[idx] * exp2f((float)exp_decode(exp_in));
-  const __half h = __float2half_rn(v);
   const size_t o = (size_t)c * ld + guard + (size_t)b * S + y * Wp + xx;
-  hi[o] = h;
-  lo[o] = __float2half_rn(v - __half2float(h));
+  split_hi_lo(x[idx] * exp2f((float)exp_decode(exp_in)), hi[o], lo[o]);
 }
 
 
@@ -169,10 +155,11 @@ __global__ void __launch_bounds__(256) k_pack_nchw(const float* __restrict__ x, 
     if (hw >= HW) continue;
     const int y = hw / W, xx = hw - y * W;
     const size_t o = ((size_t)guard + (size_t)b * S + y * Wp + xx) * cpad + c0 + 2 * tx;
-    const float v0 = t[2 * tx][ty + 8 * i], v1 = t[2 * tx + 1][ty + 8 * i];
-    const __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
+    __half h0, l0, h1, l1;
+    split_hi_lo(t[2 * tx][ty + 8 * i], h0, l0);
+    split_hi_lo(t[2 * tx + 1][ty + 8 * i], h1, l1);
     *reinterpret_cast<__half2*>(hi + o) = __halves2half2(h0, h1);
-    *reinterpret_cast<__half2*>(lo + o) = __halves2half2(__float2half_rn(v0 - __half2float(h0)), __float2half_rn(v1 - __half2float(h1)));
+    *reinterpret_cast<__half2*>(lo + o) = __halves2half2(l0, l1);
   }
 }
 // flat NHWC fp32 [guard + B*S][ld] -> NCHW [B][C][HW] (assign or accumulate); 32 x 32 tiles through shared memory
@@ -208,17 +195,12 @@ __global__ void k_prep_filter(const float* __restrict__ w, int Co, int Ci, int c
   const int kc = (int)(idx % cpad), tap = (int)((idx / cpad) % 9), row = (int)(idx / ((size_t)9 * cpad));
   float v = 0.0f;
   if (kc < kin) v = flip ? w[((size_t)kc * Ci + row) * 9 + (8 - tap)] : w[((size_t)row * Ci + kc) * 9 + tap];
-  v *= exp2f((float)exp_decode(exp_in));
-  const __half h = __float2half_rn(v);
-  hi[idx] = h;
-  lo[idx] = __float2half_rn(v - __half2float(h));
+  split_hi_lo(v * exp2f((float)exp_decode(exp_in)), hi[idx], lo[idx]);
 }
 
 // dynamic shared memory opt-in of the instantiations this file launches (per function, per device)
 void train_configure_device() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128)));
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64)));
+  set_conv_attr<256, false>(); set_conv_attr<128, false>(); set_conv_attr<64, false>();
   CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256)));
   CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128)));
   CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64)));
@@ -342,14 +324,9 @@ void tc_gemm_conv(TcGemm& g, const float* x, int Cin, const float* filter, int f
   a.n_dev = I->dB; a.n_max = I->B; a.S = I->S; a.Wp = d.W + 1; a.H = d.H; a.W = d.W; a.guard = I->guard; a.mode3d = 0; a.tps = 1;
   a.cin = cpad; a.n_total = Cout; a.cout = Cout; a.aff = nullptr; a.out_hi = nullptr; a.out_lo = nullptr; a.act_scale = 1.0f;
   a.err = nullptr; a.out_raw = I->raw; a.exp_a = sl.exp; a.exp_b = I->exp_b;
-  const int max_tiles = ((I->B * I->S + BM - 1) / BM) * (Cout / bn);
-  const int grid = std::min(I->num_sms, max_tiles);
-  auto launch = [&](auto kern, int BNv) {
-    kern<<<grid, NTHREADS, smem_bytes(BNv), st>>>(mAh, mAl, mBh, mBl, a); LAUNCH_CHECK();
-  };
-  if (bn == 256) launch(k_conv3x3_tc<256, false>, 256);
-  else if (bn == 128) launch(k_conv3x3_tc<128, false>, 128);
-  else launch(k_conv3x3_tc<64, false>, 64);
+  if (bn == 256) launch_conv<256, false>(mAh, mAl, mBh, mBl, a, I->num_sms, st);
+  else if (bn == 128) launch_conv<128, false>(mAh, mAl, mBh, mBl, a, I->num_sms, st);
+  else launch_conv<64, false>(mAh, mAl, mBh, mBl, a, I->num_sms, st);
   k_unpack_nchw<<<dim3((HW + 31) / 32, (Cout + 31) / 32, I->B), 256, 0, st>>>(I->raw, I->B, Cout, d.H, d.W, Cout, I->guard, I->S, out, accumulate ? 1 : 0); LAUNCH_CHECK();
   if (launches) *launches += nl + 4;
 }

@@ -411,17 +411,14 @@ def _c3_oracle_outputs(oracle, init, seed):
 
 
 @pytest.mark.parametrize("init,seed", [("tamed", 99), ("tamed", 7), ("reference", 5), ("reference", 11)])
-@pytest.mark.parametrize("mode", ["fp16x3-halo", "fp16x3-tap", "f8-halo", "f8-tap"])
-def test_tc_tower_full_depth_c3(oracle, engine_lib, monkeypatch, mode, init, seed):
+@pytest.mark.parametrize("mode", ["default", "fast-tower"])
+def test_tc_tower_full_depth_c3(oracle, engine_lib, mode, init, seed):
     """The headline net (20 blocks x 256, 19x19, FC 512) end to end against the oracle through all 41 conv layers, on four
     weight sets (two with the BN-scale spread of the reference's own init at batch 256: per-layer gain > 1, the nets
-    bench.py runs).  The default precision (three fp16 passes) holds the north star's 1e-4 on all of them, under every
-    kernel-selection variable a caller may set.  AZ_FLAG_FAST_TOWER may trade precision for speed, so its bound is looser
-    (this build runs the three passes for it too)."""
-    env = {"fp16x3-halo": {}, "fp16x3-tap": {"AZ_TC_HALO": "0"}, "f8-halo": {}, "f8-tap": {"AZ_TC_FP8": "1"}}[mode]
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
-    fast = mode.startswith("f8")
+    bench.py runs).  The default precision (three fp16 passes) holds the north star's 1e-4 on all of them.
+    AZ_FLAG_FAST_TOWER may trade precision for speed, so its bound is looser (this build runs the three passes for it
+    too)."""
+    fast = mode == "fast-tower"
     params, planes, po, vo = _c3_oracle_outputs(oracle, init, seed)
     d = K.make_desc(K.GAME_WQ, 19, 19, 0, komi=7.5, sims=2, n_games=4, seed=2, max_moves=4, flags=K.FLAG_FAST_TOWER if fast else 0,
                     nn=dict(k=256, shared_layers=20, fc=512, batch_size=2, features=18, action_space=362))
@@ -437,15 +434,13 @@ def test_tc_tower_full_depth_c3(oracle, engine_lib, monkeypatch, mode, init, see
     assert dp < tol and dv < tol, (mode, init, seed, dp, dv, tol)
 
 
-@pytest.mark.parametrize("mode", ["fp16x3-halo", "fp16x3-tap", "f8-halo"])
-def test_tc_tower_modes_small_nets(oracle, engine_lib, monkeypatch, mode):
-    """9x9, K = 128 (2C = 256 in the flat 2-D layout) against the oracle under each precision mode and kernel-selection
-    variable a caller may set (this build runs the three-pass wgmma kernel for all of them)."""
-    if mode == "fp16x3-tap":
-        monkeypatch.setenv("AZ_TC_HALO", "0")
+@pytest.mark.parametrize("mode", ["default", "fast-tower"])
+def test_tc_tower_modes_small_nets(oracle, engine_lib, mode):
+    """9x9, K = 128 (2C = 256 in the flat 2-D layout) against the oracle under each precision mode (this build runs the
+    three-pass wgmma kernel for both)."""
     def desc():
         return K.make_desc(K.GAME_WQ, 9, 9, 0, komi=7.5, sims=2, n_games=8, seed=2, max_moves=4,
-                           flags=K.FLAG_FAST_TOWER if mode == "f8-halo" else 0,
+                           flags=K.FLAG_FAST_TOWER if mode == "fast-tower" else 0,
                            nn=dict(k=128, shared_layers=4, fc=64, batch_size=2, features=18, action_space=82))
     eo, etc = oracle.create(desc()), engine_lib.create(desc())
     H.tame_gammas([eo, etc], 0, 13)

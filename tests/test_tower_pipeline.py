@@ -12,7 +12,8 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "agogo_b200", "libagogo_b200.so")
 GOLDEN = os.path.join(ROOT, "tests", "golden", "tower_c3_bits.npz")
-K_STEPS_PER_BLOCK = 4  # k_conv3x3_tc's K block is 64 channels: four k16 wgmma steps
+K_STEPS_PER_BLOCK = 4  # a K block of the wgmma kernels is 64 channels: four k16 wgmma steps
+TC_PASSES = 3  # the pass count of every tensor-core kernel but the diagnostic k_conv3x3_tc instantiations
 
 
 def _cuobjdump():
@@ -32,18 +33,28 @@ def _sass_functions(tool):
     return funcs
 
 
+def _passes(name):
+    """Tensor passes per K block of a wgmma kernel, or None for any other function."""
+    if "k_conv3x3_tc" in name:
+        m = re.search(r"k_conv3x3_tcILi(\d+)ELb([01])ELi(\d)E", name)
+        assert m, name
+        return int(m.group(3))
+    return TC_PASSES if "k_dw_tc" in name or "k_net_small" in name else None
+
+
 def test_conv_kernel_one_warpgroup_arrive_per_k_block():
-    """Every k_conv3x3_tc instantiation issues each K block as one batch: one WARPGROUP.ARRIVE, then all
-    passes x k16 HGMMAs with nothing in between, and only the last one waits on the scoreboard (gsb0)."""
+    """Every wgmma kernel (each k_conv3x3_tc and k_dw_tc instantiation, and k_net_small with one K-block loop per layer
+    width) issues each K block as one batch: one WARPGROUP.ARRIVE, then all passes x k16 HGMMAs with nothing in between,
+    and only the last one waits on the scoreboard (gsb0)."""
     tool = _cuobjdump()
     if not os.path.exists(LIB) or tool is None:
         pytest.skip("needs the built library and cuobjdump")
-    convs = {n: body for n, body in _sass_functions(tool).items() if "k_conv3x3_tc" in n}
-    assert convs, "no k_conv3x3_tc in the library"
-    for name, body in convs.items():
-        m = re.search(r"k_conv3x3_tcILi(\d+)ELb([01])ELi(\d)E", name)
-        assert m, name
-        passes = int(m.group(3))
+    kernels = {n: (_passes(n), body) for n, body in _sass_functions(tool).items() if _passes(n) is not None}
+    names = " ".join(kernels)
+    assert "k_conv3x3_tc" in names, "no k_conv3x3_tc in the library"
+    for kernel in ("k_dw_tcILi64E", "k_dw_tcILi128E", "k_dw_tcILi256E", "k_net_small"):
+        assert kernel in names, "no %s in the library" % kernel
+    for name, (passes, body) in kernels.items():
         ins = [ln for ln in body if "WARPGROUP.ARRIVE" in ln or "HGMMA" in ln]
         arrives = sum("WARPGROUP.ARRIVE" in ln for ln in ins)
         hgmma = [ln for ln in ins if "HGMMA" in ln]
