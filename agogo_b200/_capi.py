@@ -66,6 +66,7 @@ SYMBOLS = [
     "az_game_state", "az_examples_count", "az_examples_read", "az_examples_clear", "az_tree_dump", "az_rules_apply",
     "az_rules_status", "az_train", "az_comm_unique_id", "az_comm_init", "az_counters_get", "az_counters_reset",
     "az_build_info", "az_profile", "az_train_grads", "az_train_apply", "az_search", "az_comm_bench", "az_agent_reset_tree",
+    "az_infer_tower",
 ]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -191,6 +192,15 @@ class Engine:
         val = np.empty(n, np.float32)
         self._ck(self.lib.dll.az_infer(self.h, agent, _p(planes, C.c_float), n, _p(pol, C.c_float), _p(val, C.c_float)))
         return pol, val
+
+    def infer_tower(self, agent, planes):
+        """The residual tower's output for the same forward as infer(): [n, K, H, W] fp32 (diagnostics)."""
+        planes = np.ascontiguousarray(planes, np.float32).reshape(-1, self.plane)
+        n = planes.shape[0]
+        nn = self.desc.nn
+        out = np.empty((n, nn.k, nn.height, nn.width), np.float32)
+        self._ck(self.lib.dll.az_infer_tower(self.h, agent, _p(planes, C.c_float), n, _p(out, C.c_float)))
+        return out
 
     def stats(self, agent):
         w, l, d = C.c_float(), C.c_float(), C.c_float()

@@ -461,17 +461,18 @@ int az_agent_set_table(az_engine* e, int32_t agent, int32_t n_rows, int32_t row_
   return AZ_OK;
 }
 
-// forward of one agent's pending batch (count on device)
-static void run_forward(az_engine* e, int agent, cudaStream_t st = nullptr) {
+// forward of one agent's pending batch (count on device); returns the fp32 tower's output buffer (nullptr on the
+// tensor-core tower, whose output stays in its own fp16 hi/lo layout)
+static const float* run_forward(az_engine* e, int agent, cudaStream_t st = nullptr) {
   if (!st) st = e->stream;
   const EngineDev& E = e->E;
-  if (E.inf[agent].kind != INF_DUAL) return;
+  if (E.inf[agent].kind != INF_DUAL) return nullptr;
   const float* in = E.nn_in + (size_t)agent * E.GS * e->P.plane;
   float* pol = E.policy + (size_t)agent * E.GS * E.Lmax;
   float* val = E.value + (size_t)agent * E.GS;
   const int* cnt = E.batch_count + agent;
-  if (e->use_tc) tc_tower_forward(e->tc[agent], e->L, e->snap[agent], e->fp32, in, cnt, E.GS, pol, E.Lmax, val, E.err, st, &e->launches);
-  else forward_fp32(e->L, e->snap[agent], e->fp32, in, cnt, E.GS, pol, E.Lmax, val, st, &e->launches);
+  if (e->use_tc) { tc_tower_forward(e->tc[agent], e->L, e->snap[agent], e->fp32, in, cnt, E.GS, pol, E.Lmax, val, E.err, st, &e->launches); return nullptr; }
+  return forward_fp32(e->L, e->snap[agent], e->fp32, in, cnt, E.GS, pol, E.Lmax, val, st, &e->launches);
 }
 
 int az_infer(az_engine* e, int32_t agent, const float* planes, int32_t n, float* policy, float* value) {
@@ -491,6 +492,33 @@ int az_infer(az_engine* e, int32_t agent, const float* planes, int32_t n, float*
     CUDA_CHECK(cudaMemcpy2DAsync(policy + (size_t)done * A1, (size_t)A1 * 4, E.policy + (size_t)agent * E.GS * E.Lmax,
                                  (size_t)E.Lmax * 4, (size_t)A1 * 4, chunk, cudaMemcpyDeviceToHost, e->stream));
     CUDA_CHECK(cudaMemcpyAsync(value + done, E.value + (size_t)agent * E.GS, (size_t)chunk * 4, cudaMemcpyDeviceToHost, e->stream));
+    CUDA_CHECK(cudaStreamSynchronize(e->stream));
+  }
+  int bits = 0;
+  CUDA_CHECK(cudaMemcpy(&bits, E.err, 4, cudaMemcpyDeviceToHost));
+  if (bits) { CUDA_CHECK(cudaMemsetAsync(E.err, 0, 4, e->stream)); return device_error_to_rc(e, bits); }
+  GUARD_END(e)
+  return AZ_OK;
+}
+int az_infer_tower(az_engine* e, int32_t agent, const float* planes, int32_t n, float* tower_out) {
+  if (agent < 0 || agent > 1 || n < 0) return AZ_ERR_INVALID;
+  if (e->E.inf[agent].kind != INF_DUAL || !e->snap_valid[agent]) { e->err = "agent has no dual inferer (call az_agent_set_inferer(AZ_INF_DUAL))"; return AZ_ERR_STATE; }
+  if (e->in_play) { e->err = "az_infer_tower during a running arena"; return AZ_ERR_STATE; }
+  GUARD_BEGIN
+  CUDA_CHECK(cudaSetDevice(e->device));
+  const EngineDev& E = e->E;
+  const size_t per = (size_t)e->L.d.K * e->L.d.HW();
+  for (int done = 0; done < n; done += E.GS) {
+    int chunk = std::min(E.GS, n - done);
+    CUDA_CHECK(cudaMemcpyAsync(E.nn_in + (size_t)agent * E.GS * e->P.plane, planes + (size_t)done * e->P.plane,
+                               (size_t)chunk * e->P.plane * 4, cudaMemcpyHostToDevice, e->stream));
+    CUDA_CHECK(cudaMemcpyAsync(E.batch_count + agent, &chunk, 4, cudaMemcpyHostToDevice, e->stream));
+    const float* tower = run_forward(e, agent);
+    if (e->use_tc) {  // the fp32 tower's scratch is idle on this engine: unpack the hi/lo output into it
+      tc_tower_output(e->tc[agent], E.batch_count + agent, E.GS, e->fp32.a, e->stream);
+      tower = e->fp32.a;
+    }
+    CUDA_CHECK(cudaMemcpyAsync(tower_out + (size_t)done * per, tower, (size_t)chunk * per * 4, cudaMemcpyDeviceToHost, e->stream));
     CUDA_CHECK(cudaStreamSynchronize(e->stream));
   }
   int bits = 0;

@@ -52,12 +52,12 @@ void snapshot_gather(const NetLayout& L, const float* params_dev, Snapshot& s, c
 
 // fp32 CUDA-core forward (validation-grade, op order identical to the oracle's):
 //   planes [n, F, H, W] (device) -> policy [n, ldp] (first A1 entries), value [n]
-// n is read from *n_dev (device) and clamped to n_max.
+// n is read from *n_dev (device) and clamped to n_max.  Returns the tower output it handed to the heads (dense NCHW, in sc).
 struct Fp32Scratch { float *a = nullptr, *b = nullptr, *ph = nullptr, *vh = nullptr; size_t cap = 0; };
 void fp32_scratch_alloc(Fp32Scratch& s, const NetDims& d, int n_max);
 void fp32_scratch_free(Fp32Scratch& s);
-void forward_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const float* planes, const int* n_dev, int n_max,
-                  float* policy, int ldp, float* value, cudaStream_t st, unsigned long long* launches);
+const float* forward_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const float* planes, const int* n_dev, int n_max,
+                          float* policy, int ldp, float* value, cudaStream_t st, unsigned long long* launches);
 // heads only, from a dense fp32 NCHW tower output
 void heads_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const float* tower, const int* n_dev, int n_max,
                 float* policy, int ldp, float* value, cudaStream_t st, unsigned long long* launches);

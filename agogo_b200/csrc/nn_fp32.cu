@@ -357,8 +357,8 @@ void heads_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const fl
   if (launches) (*launches)++;
 }
 
-void forward_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const float* planes, const int* n_dev, int n_max,
-                  float* policy, int ldp, float* value, cudaStream_t st, unsigned long long* launches) {
+const float* forward_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const float* planes, const int* n_dev, int n_max,
+                          float* policy, int ldp, float* value, cudaStream_t st, unsigned long long* launches) {
   const NetDims& d = L.d;
   float* cur = sc.a;
   float* nxt = sc.b;
@@ -369,4 +369,5 @@ void forward_fp32(const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const 
     float* t = cur; cur = nxt; nxt = t;
   }
   heads_fp32(L, s, sc, cur, n_dev, n_max, policy, ldp, value, st, launches);
+  return cur;
 }

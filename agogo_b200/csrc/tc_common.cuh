@@ -223,9 +223,14 @@ __device__ __forceinline__ uint64_t make_desc_mn_sw128(uint32_t smem_addr, uint3
   return d;
 }
 
-// training operands carry a data-dependent power-of-two scale: the device word is ilogb(absmax) - 13 (or the
+// training operands carry a data-dependent power-of-two scale: the device word is max(ilogb(absmax) - 13, -127) (or the
 // 0x80808080 fill when the tensor is all zero); scale exponent e = -word
 __device__ __forceinline__ int exp_decode(const int* e) { const int v = *e; return v < -100000 ? 0 : -v; }
+// v * 2^-e rounded once, as ldexpf(v, -e): one multiply while 2^-e is a normal float (e is the same for every thread, so
+// the branch is uniform); ldexpf once 2^-e alone would flush to zero while the product is still a float
+__device__ __forceinline__ float descale(float v, int e) {
+  return e >= -127 && e <= 126 ? v * __int_as_float((127 - e) << 23) : ldexpf(v, -e);
+}
 
 struct ConvArgs {
   const int* n_dev;   // batch size (device)
@@ -384,11 +389,11 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
       const bool valid = inb && y < a.H && x < a.W;
       if (!valid) continue;
       if (a.out_raw) {
-        const float sc = exp2f(-(float)(exp_decode(a.exp_a) + exp_decode(a.exp_b)));
+        const int e = exp_decode(a.exp_a) + exp_decode(a.exp_b);
         float* o = a.out_raw + (size_t)(a.guard + r) * a.n_total + n0 + col0;
 #pragma unroll
         for (int j = 0; j < BN / 8; j++)
-          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[4 * j + 2 * h] * sc, acc[4 * j + 2 * h + 1] * sc);
+          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(descale(acc[4 * j + 2 * h], e), descale(acc[4 * j + 2 * h + 1], e));
         continue;
       }
       const int hw = y * a.W + x;

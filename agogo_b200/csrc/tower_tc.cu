@@ -92,6 +92,18 @@ __global__ void k_head_convs_nhwc(const __half* __restrict__ hi, const __half* _
     vh[(size_t)b * HW + hw] = v0 > 0.0f ? v0 : 0.0f;
   }
 }
+// diagnostics: the NHWC hi/lo tower output (the values k_head_convs_nhwc reads) -> fp32 NCHW [n][K][HW]
+__global__ void k_tower_nchw(const __half* __restrict__ hi, const __half* __restrict__ lo, const int* __restrict__ n_dev, int n_max,
+                             int K, int H, int W, int guard, int S, float inv_scale, float* out) {
+  const int n = min(*n_dev, n_max);
+  const int HW = H * W, Wp = W + 1;
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (size_t)n * K * HW) return;
+  const int hw = (int)(idx % HW), c = (int)((idx / HW) % K), b = (int)(idx / ((size_t)HW * K));
+  const int y = hw / W, x = hw - y * W;
+  const size_t o = ((size_t)guard + (size_t)b * S + y * Wp + x) * K + c;
+  out[idx] = (__half2float(hi[o]) + __half2float(lo[o])) * inv_scale;
+}
 
 // -------------------------------------------------------------------------------------------------
 // k_net_small: the whole tower of a K = 64 net on a board of at most 128 padded positions ((H+1)(W+1) <= 128, BASELINE
@@ -456,6 +468,17 @@ void tc_tower_forward(TcTower& t, const NetLayout& NL, const Snapshot& s, Fp32Sc
   }
   heads_tiled(NL, s, sc.ph, sc.vh, n_dev, n_max, policy, ldp, value, st, launches);
   if (I->profile) I->fwd_spans.push_back({f0, I->ev_get(st)});
+}
+
+void tc_tower_output(TcTower& t, const int* n_dev, int n_max, float* out, cudaStream_t st) {
+  const Impl* I = (const Impl*)t.impl;
+  if (!I || !t.ready) throw std::runtime_error("tc tower not prepared");
+  const NetDims& d = I->d;
+  // k_net_small leaves the last layer in buffer 0; the per-layer path swaps buffers once per fused layer
+  const int last = I->small ? 0 : (int)(I->layers.size() - 1) & 1;
+  const size_t total = (size_t)n_max * d.K * d.HW();
+  k_tower_nchw<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(I->x_hi[last], I->x_lo[last], n_dev, n_max, d.K, d.H, d.W, I->guard,
+                                                                I->S, ldexpf(1.0f, -I->ea), out); LAUNCH_CHECK();
 }
 
 void tc_tower_profile(TcTower& t, bool enable) {

@@ -23,6 +23,8 @@ void tc_tower_profile_collect(TcTower& t, cudaStream_t st, double* conv_ms, doub
 void tc_tower_forward(TcTower& t, const NetLayout& L, const Snapshot& s, Fp32Scratch& sc, const float* planes,
                       const int* n_dev, int n_max, float* policy, int ldp, float* value, int* err_flag, cudaStream_t st,
                       unsigned long long* launches);
+// diagnostics: the tower output of the last tc_tower_forward (the buffer the head convs read) as fp32 NCHW out [n][K][H][W]
+void tc_tower_output(TcTower& t, const int* n_dev, int n_max, float* out, cudaStream_t st);
 
 // K7: the 3x3 convolutions of the training pass (forward, backward-data, backward-filter) on wgmma (train_tc.cu)
 struct TcGemm { void* impl = nullptr; };

@@ -95,12 +95,12 @@ __global__ void k_dw_reduce(const float* __restrict__ partial, int splits, int C
                             const int* __restrict__ eb, float* __restrict__ dW) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= Co * Ci) return;
-  const float sc = exp2f(-(float)(exp_decode(ea) + exp_decode(eb)));
+  const int e = exp_decode(ea) + exp_decode(eb);
   const size_t tap_stride = (size_t)Co * Ci;
   for (int tap = 0; tap < 9; tap++) {
     float acc = 0.0f;
     for (int sp = 0; sp < splits; sp++) acc += partial[(size_t)(sp * 9 + tap) * tap_stride + idx];
-    dW[(size_t)idx * 9 + tap] = acc * sc;
+    dW[(size_t)idx * 9 + tap] = descale(acc, e);
   }
 }
 // NCHW fp32 [B][C][HW] -> channel-major hi/lo [C][ld] at column guard + b*S + y*(W+1) + x, scaled by 2^(*exp)
@@ -128,8 +128,9 @@ __global__ void k_absmax_exp(const float* __restrict__ x, size_t n, int* exp_out
     m = threadIdx.x < (blockDim.x >> 5) ? sh[threadIdx.x] : 0.0f;
 #pragma unroll
     for (int off = 16; off; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
-    // scale so that the largest magnitude lands in [2^13, 2^14): hi below fp16 overflow, lo as far from underflow as possible
-    if (threadIdx.x == 0) atomicMax(exp_out, (m > 0.0f && isfinite(m)) ? ilogbf(m) - 13 : -0x7fffffff);  // stores -e (max over blocks)
+    // scale so that the largest magnitude lands in [2^13, 2^14): hi below fp16 overflow, lo as far from underflow as possible.
+    // The scale 2^e must itself be a finite float (e <= 127): a tensor below 2^-114 lands lower, instead of 0 * inf = NaN.
+    if (threadIdx.x == 0) atomicMax(exp_out, (m > 0.0f && isfinite(m)) ? max(ilogbf(m) - 13, -127) : -0x7fffffff);  // stores -e (max over blocks)
   }
 }
 

@@ -121,7 +121,8 @@ typedef struct az_engine_desc {
   uint32_t flags;
   uint64_t seed;    /* replaces the reference's time.Now() seeds (arena.go:61, tree.go:84) */
   int32_t act_scale_log2;     /* tensor-core tower: activations are stored as fp16 hi/lo of x*2^this; 0 = default (-2: |x| up to 2.6e5
-                               * before AZ_ERR_PANIC "activation overflow"; outputs are insensitive to it between -5 and 5) */
+                               * before AZ_ERR_PANIC "activation overflow"; between -5 and 5 the outputs agree to the storage's
+                               * resolution: |x| below 2^-(3+this) is kept to an absolute 2^-(25+this)) */
   int32_t max_nodes_per_tree; /* 0 = derive from sims and action space */
 } az_engine_desc;
 
@@ -152,6 +153,11 @@ int az_agent_set_table(az_engine* e, int32_t agent, int32_t n_rows, int32_t row_
 /* Agent.NNOutput / Inferer.Infer (agent.go:83-89, meta.go:168-190) batched: planes [n,F,H,W]
  * -> policy [n,action_space], value [n].  Uses the agent's inference snapshot. */
 int az_infer(az_engine* e, int32_t agent, const float* planes, int32_t n, float* policy, float* value);
+/* Diagnostics: the same forward as az_infer, but returns the residual tower's output — the activations the policy and value
+ * head convs read — as fp32 tower_out [n,K,H,W].  On the tensor-core tower that is the stored fp16 hi/lo pair,
+ * (hi + lo) / 2^act_scale_log2.  Lets a test compare one conv layer at a time: a net with SharedLayers = l computes the
+ * first l blocks of a deeper net with the same leading weights. */
+int az_infer_tower(az_engine* e, int32_t agent, const float* planes, int32_t n, float* tower_out);
 int az_agent_stats(const az_engine* e, int32_t agent, float* wins, float* loss, float* draw);
 int az_agent_reset_stats(az_engine* e, int32_t agent); /* agent.go:115-121 */
 

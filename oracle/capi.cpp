@@ -159,6 +159,17 @@ int az_infer(az_engine* e, int32_t agent, const float* planes, int32_t n, float*
   GUARD_END(e)
   return AZ_OK;
 }
+int az_infer_tower(az_engine* e, int32_t agent, const float* planes, int32_t n, float* tower_out) {
+  if (agent < 0 || agent > 1 || n < 0) return AZ_ERR_INVALID;
+  DualInferer* di = dynamic_cast<DualInferer*>(e->inferers[agent].get());
+  if (!di) { e->err = "agent has no dual inferer (call az_agent_set_inferer(AZ_INF_DUAL))"; return AZ_ERR_STATE; }
+  GUARD_BEGIN
+  std::vector<float> policy((size_t)n * di->net.conf.ActionSpace), value(n), tower;
+  dual_infer(di->net, planes, n, policy.data(), value.data(), &tower);
+  std::copy(tower.begin(), tower.end(), tower_out);
+  GUARD_END(e)
+  return AZ_OK;
+}
 int az_agent_stats(const az_engine* e, int32_t agent, float* wins, float* loss, float* draw) {
   if (agent < 0 || agent > 1) return AZ_ERR_INVALID;
   *wins = e->wins[agent]; *loss = e->loss[agent]; *draw = e->draw[agent];

@@ -34,7 +34,7 @@ def conv(x, w):  # cross-correlation, stride 1, same padding (findPadding), no b
     out = np.zeros((B, w.shape[0], H, W))
     for ky in range(k):
         for kx in range(k):
-            out += np.einsum("oc,bchw->bohw", w[:, :, ky, kx], xp[:, :, ky:ky + H, kx:kx + W])
+            out += np.tensordot(w[:, :, ky, kx], xp[:, :, ky:ky + H, kx:kx + W], axes=(1, 1)).transpose(1, 0, 2, 3)
     return out
 
 
@@ -98,6 +98,12 @@ class Net:
             s = self.units[1 + 2 * i].fwd(cur, train) + self.units[2 + 2 * i].fwd(cur, train)
             self.sums.append(s)
             cur = np.maximum(s, 0)
+        self.tower = cur
+        return self.heads(cur, train)
+
+    def heads(self, cur, train):
+        """policy logits and pre-tanh value from the tower output cur [B,K,H,W]"""
+        B = cur.shape[0]
         self.ph = self.pu.fwd(cur, train).reshape(B, -1)
         self.logits = self.ph @ self.pw + (self.pb if train else self.pb[0])
         self.vh = self.vu.fwd(cur, train).reshape(B, -1)
@@ -106,8 +112,9 @@ class Net:
         self.vraw = (self.h1 @ self.ow + (self.ob if train else self.ob[0])).reshape(B)
         return self.logits, self.vraw
 
-    def infer(self, X):
-        logits, vraw = self.forward(X, False)
+    def infer(self, X=None, tower=None):
+        """softmax policy and tanh value of the planes X, or of the heads alone applied to a given tower output"""
+        logits, vraw = self.forward(X, False) if tower is None else self.heads(tower, False)
         ex = np.exp(logits)
         return ex / ex.sum(axis=1, keepdims=True), np.tanh(vraw)
 

@@ -40,3 +40,8 @@ def test_dual_forward_and_gradients_vs_numpy(oracle, kind, m, n, k, nn):
     po, vo = e.infer(0, Xi.astype(np.float32).reshape(5, -1))
     pn, vn = net0.infer(Xi)
     assert np.abs(po - pn).max() < 2e-5 and np.abs(vo - vn).max() < 2e-5, (np.abs(po - pn).max(), np.abs(vo - vn).max())
+    # ---- the tower output (az_infer_tower): NCHW [n,K,H,W], the activations the heads read
+    to = e.infer_tower(0, Xi.astype(np.float32).reshape(5, -1))
+    tn = net0.tower
+    assert to.shape == tn.shape == (5, nn["k"], m, n), (to.shape, tn.shape)
+    assert np.abs(to - tn).max() <= 1e-6 * np.abs(tn).max(), (np.abs(to - tn).max(), np.abs(tn).max())
