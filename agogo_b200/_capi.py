@@ -17,6 +17,7 @@ GAME_MNK, GAME_C4, GAME_WQ = 0, 1, 2
 ENC_TWO_PLANE, ENC_WQ18 = 0, 1
 INF_DUAL, INF_DUMMY, INF_TABLE = 0, 1, 2
 FLAG_SHARED_TREE, FLAG_FP32_TOWER, FLAG_FAST_TOWER, FLAG_WQ_COMPLETE = 1, 2, 4, 8
+FLAG_FP16_TOWER = 16  # one fp16 per operand, one tensor pass, looser precision contract (include/agogo_b200.h)
 DONT_PREFER_PASS, PREFER_PASS, DONT_RESIGN = 0, 1, 2
 
 

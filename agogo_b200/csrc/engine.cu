@@ -341,9 +341,11 @@ int az_engine_create(const az_engine_desc* desc, az_engine** out) {
       e->snap[a].d = e->dalloc<float>(e->snap[a].total);
     }
     fp32_scratch_alloc(e->fp32, nd, E.GS);
+    // AZ_FLAG_FP32_TOWER wins over AZ_FLAG_FP16_TOWER, which wins over AZ_FLAG_FAST_TOWER (the three-pass kernels)
     e->use_tc = !(desc->flags & AZ_FLAG_FP32_TOWER) && tc_tower_supported(nd);
     if (e->use_tc)
-      for (int a = 0; a < 2; a++) tc_tower_alloc(e->tc[a], nd, E.GS, desc->act_scale_log2 ? desc->act_scale_log2 : -2);
+      for (int a = 0; a < 2; a++)
+        tc_tower_alloc(e->tc[a], nd, E.GS, desc->act_scale_log2 ? desc->act_scale_log2 : -2, (desc->flags & AZ_FLAG_FP16_TOWER) != 0);
 
     CUDA_CHECK(cudaMallocHost(&e->h_ex_board, (size_t)G * P.plane * 4));
     CUDA_CHECK(cudaMallocHost(&e->h_ex_policy, (size_t)G * (P.A + 1) * 4));

@@ -32,9 +32,19 @@ constexpr int CONSUMER_WARPS = 8;
 constexpr int TC_PASSES = 3;   // hi*hi + hi*lo + lo*hi (fp32-faithful); 2 drops lo*hi, 1 is hi*hi only (diagnostics)
 // H100: 227 KB of dynamic shared memory per block, less alignment slack and the barriers
 constexpr int SMEM_RING_BUDGET = 227 * 1024 - 2048;
-__host__ __device__ constexpr int stage_bytes(int BN) { return 2 * BM * BK * 2 + 2 * BN * BK * 2; }
-__host__ __device__ constexpr int num_stages(int BN) { return SMEM_RING_BUDGET / stage_bytes(BN) > 8 ? 8 : SMEM_RING_BUDGET / stage_bytes(BN); }
-__host__ __device__ constexpr int smem_bytes(int BN) { return num_stages(BN) * stage_bytes(BN) + 1024 + 256; }
+// OPS: fp16 planes stored per operand — 2 = hi/lo (fp32-faithful), 1 = one fp16 (AZ_FLAG_FP16_TOWER)
+__host__ __device__ constexpr int stage_bytes(int BN, int OPS = 2) { return OPS * (BM * BK * 2 + BN * BK * 2); }
+__host__ __device__ constexpr int num_stages(int BN, int OPS = 2) {
+  return SMEM_RING_BUDGET / stage_bytes(BN, OPS) > 8 ? 8 : SMEM_RING_BUDGET / stage_bytes(BN, OPS);
+}
+__host__ __device__ constexpr int smem_bytes(int BN, int OPS = 2) { return num_stages(BN, OPS) * stage_bytes(BN, OPS) + 1024 + 256; }
+
+// The stored fp16 planes of an operand, and the tensor maps over them: hi and lo for the fp32-faithful form, hi alone for
+// the fp16 form, so that a kernel instantiated for one plane has no lo to read or write.
+template <int OPS> struct Planes { __half *hi, *lo; };
+template <> struct Planes<1> { __half* hi; };
+template <int OPS> struct PlaneMaps { CUtensorMap hi, lo; };
+template <> struct PlaneMaps<1> { CUtensorMap hi; };
 
 // The operand format of every tensor-core pass: v = hi + lo, hi = fp16(v), lo = fp16(v - hi).  Callers scale v by a
 // power of two first so that lo stays a normal fp16.
@@ -242,8 +252,6 @@ struct ConvArgs {
   int n_total;        // GEMM N of the layer (fused: 2*K)
   int cout;           // output channels (K)
   const float2* aff;  // [HW][n_total] {A', B} in weight-row order
-  __half* out_hi;     // [(guard + rows)][cout]
-  __half* out_lo;
   float act_scale;    // 2^ea
   int* err;
   // raw mode (training, K7): no affine / ReLU / split — the epilogue writes acc * 2^-(*exp_a + *exp_b) as fp32
@@ -299,13 +307,17 @@ __host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n) {
   return a.mode3d ? n * a.tps : (n * a.S + BM - 1) / BM;
 }
 
-template <int BN, bool PAIR, int PASSES = TC_PASSES>
+// OPS = 2: activations and filters as fp16 hi/lo planes (out: hi/lo, or raw fp32 for training).  OPS = 1: one fp16
+// plane each, one pass (PASSES = 1), the output rounded once to fp16; half the bytes per stage, so a deeper ring.
+// Stage layout: A planes, then B planes.
+template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
 __global__ void __launch_bounds__(NTHREADS, 1)
-k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-             const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo, ConvArgs a) {
+k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__ PlaneMaps<OPS> tmB, ConvArgs a,
+             Planes<OPS> out) {
+  static_assert(OPS == 2 || PASSES == 1, "a single fp16 plane has one pass");
   constexpr int A_TILE_BYTES = BM * BK * 2;
-  constexpr int STAGES = num_stages(BN);
-  constexpr int STAGE_BYTES = stage_bytes(BN);
+  constexpr int STAGES = num_stages(BN, OPS);
+  constexpr int STAGE_BYTES = stage_bytes(BN, OPS);
   constexpr int B_TILE_BYTES = BN * BK * 2;
   constexpr int OUTC = PAIR ? BN / 2 : BN;  // output channels per N tile
   extern __shared__ uint8_t smem_raw[];
@@ -337,15 +349,15 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
           const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES, bar = ring.full(it);
           if (a.mode3d) {
             const int b = mt / a.tps, p0 = (mt - b * a.tps) * BM + dy * a.Wp + dx;  // may be <0 / >=S: zero fill
-            tma_load_3d(sa, &tmA_hi, bar, kc * BK, p0, b);
-            tma_load_3d(sa + A_TILE_BYTES, &tmA_lo, bar, kc * BK, p0, b);
+            tma_load_3d(sa, &tmA.hi, bar, kc * BK, p0, b);
+            if constexpr (OPS == 2) tma_load_3d(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, p0, b);
           } else {
             const int arow = a.guard + m0 + dy * a.Wp + dx;
-            tma_load_2d(sa, &tmA_hi, bar, kc * BK, arow);
-            tma_load_2d(sa + A_TILE_BYTES, &tmA_lo, bar, kc * BK, arow);
+            tma_load_2d(sa, &tmA.hi, bar, kc * BK, arow);
+            if constexpr (OPS == 2) tma_load_2d(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, arow);
           }
-          tma_load_2d(sa + 2 * A_TILE_BYTES, &tmB_hi, bar, tap * a.cin + kc * BK, n0);
-          tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB_lo, bar, tap * a.cin + kc * BK, n0);
+          tma_load_2d(sa + OPS * A_TILE_BYTES, &tmB.hi, bar, tap * a.cin + kc * BK, n0);
+          if constexpr (OPS == 2) tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB.lo, bar, tap * a.cin + kc * BK, n0);
         }
       }
     }
@@ -363,9 +375,12 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
     for (int kb = 0; kb < kblocks; kb++, it++) {
       ring.consumer_wait(it);
       const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES;
-      mma_kblock<BN, 0, PASSES>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
-                                make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
-                                kb == 0);
+      if constexpr (OPS == 2)
+        mma_kblock<BN, 0, PASSES>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
+                                  make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
+                                  kb == 0);
+      else
+        mma_kblock<BN, 0, 1>(acc, make_desc_sw(sa + wg * 64 * 128), 0, make_desc_sw(sa + A_TILE_BYTES), 0, 32 >> 4, kb == 0);
       ring.consumer_release(it);
     }
     // ===== epilogue from registers =====
@@ -388,28 +403,31 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
       const int y = p / a.Wp, x = p - y * a.Wp;
       const bool valid = inb && y < a.H && x < a.W;
       if (!valid) continue;
-      if (a.out_raw) {
-        const int e = exp_decode(a.exp_a) + exp_decode(a.exp_b);
-        float* o = a.out_raw + (size_t)(a.guard + r) * a.n_total + n0 + col0;
+      if constexpr (OPS == 2) {
+        if (a.out_raw) {
+          const int e = exp_decode(a.exp_a) + exp_decode(a.exp_b);
+          float* o = a.out_raw + (size_t)(a.guard + r) * a.n_total + n0 + col0;
 #pragma unroll
-        for (int j = 0; j < BN / 8; j++)
-          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(descale(acc[4 * j + 2 * h], e), descale(acc[4 * j + 2 * h + 1], e));
-        continue;
+          for (int j = 0; j < BN / 8; j++)
+            *reinterpret_cast<float2*>(o + 8 * j) = make_float2(descale(acc[4 * j + 2 * h], e), descale(acc[4 * j + 2 * h + 1], e));
+          continue;
+        }
       }
       const int hw = y * a.W + x;
       const float2* aff = a.aff + (size_t)hw * a.n_total + n0 + col0;
-      __half* ohi = a.out_hi + (size_t)(a.guard + r) * a.cout + nt * OUTC + col0;
-      __half* olo = a.out_lo + (size_t)(a.guard + r) * a.cout + nt * OUTC + col0;
+      const size_t o = (size_t)(a.guard + r) * a.cout + nt * OUTC + col0;
 #pragma unroll
       for (int j = 0; j < OUTC / 8; j++) {
         __half hv[2], lv[2];
 #pragma unroll
         for (int e = 0; e < 2; e++) {
-          split_hi_lo(fused_value<BN, PAIR>(aff, acc, j, h, e, a.act_scale), hv[e], lv[e]);
+          const float v = fused_value<BN, PAIR>(aff, acc, j, h, e, a.act_scale);
+          if constexpr (OPS == 2) split_hi_lo(v, hv[e], lv[e]);
+          else hv[e] = __float2half_rn(v);
           overflow |= !(fabsf(__half2float(hv[e])) <= 65504.0f);
         }
-        *reinterpret_cast<__half2*>(ohi + 8 * j) = __halves2half2(hv[0], hv[1]);
-        *reinterpret_cast<__half2*>(olo + 8 * j) = __halves2half2(lv[0], lv[1]);
+        *reinterpret_cast<__half2*>(out.hi + o + 8 * j) = __halves2half2(hv[0], hv[1]);
+        if constexpr (OPS == 2) *reinterpret_cast<__half2*>(out.lo + o + 8 * j) = __halves2half2(lv[0], lv[1]);
       }
     }
     if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
@@ -417,16 +435,17 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__
 }
 
 // dynamic shared memory opt-in of one instantiation on the current device (the attribute is per function and per device)
-template <int BN, bool PAIR, int PASSES = TC_PASSES>
+template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
 void set_conv_attr() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, PASSES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(BN)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, PASSES, OPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  smem_bytes(BN, OPS)));
 }
 // persistent grid: one CTA per SM, or one per tile when the largest batch has fewer
-template <int BN, bool PAIR, int PASSES = TC_PASSES>
-void launch_conv(const CUtensorMap& ah, const CUtensorMap& al, const CUtensorMap& bh, const CUtensorMap& bl, const ConvArgs& a,
-                 int num_sms, cudaStream_t st) {
+template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
+void launch_conv(const PlaneMaps<OPS>& A, const PlaneMaps<OPS>& B, const ConvArgs& a, const Planes<OPS>& out, int num_sms,
+                 cudaStream_t st) {
   const int grid = std::min(num_sms, conv_m_tiles(a, a.n_max) * (a.n_total / BN));
-  k_conv3x3_tc<BN, PAIR, PASSES><<<grid, NTHREADS, smem_bytes(BN), st>>>(ah, al, bh, bl, a); LAUNCH_CHECK();
+  k_conv3x3_tc<BN, PAIR, PASSES, OPS><<<grid, NTHREADS, smem_bytes(BN, OPS), st>>>(A, B, a, out); LAUNCH_CHECK();
 }
 
 // ---------------------------------------------------------------------------------------------

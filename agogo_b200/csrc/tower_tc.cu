@@ -14,7 +14,8 @@
 //     TMA, M-tiles never straddle samples (19x19: 3 tiles = 384 rows per 361 points vs 400);
 //   * fp32 fidelity on fp16 tensor cores: x = hi + lo and w = hi + lo (both pre-scaled by powers of
 //     two), three wgmma passes per K-step (hi*hi + hi*lo + lo*hi) into one fp32 register
-//     accumulator; the dropped lo*lo term is ~2^-22 relative;
+//     accumulator; the dropped lo*lo term is ~2^-22 relative.  Under AZ_FLAG_FP16_TOWER the same
+//     kernels are instantiated for one fp16 plane per operand (OPS = 1): one pass, no lo buffers;
 //   * warp roles (tc_common.cuh): one TMA producer warp, two consumer warpgroups of 64 rows each;
 //     smem ring of K-blocks (full/empty mbarriers), persistent CTAs striding over (M-tile, N-tile),
 //     epilogue (BN-affine + ReLU + branch add -> fp16 hi/lo split -> global) from the accumulators.
@@ -29,9 +30,17 @@ __device__ __forceinline__ float plane_input(const float* planes, int F, int HW,
   return on_board && c < F ? planes[((size_t)b * F + c) * HW + hw] * scale : 0.0f;
 }
 
-// fp32 NCHW planes -> zero-bordered NHWC fp16 hi/lo (channels padded to cpad)
+// a stored activation in fp32: hi + lo, or the single fp16
+template <int OPS>
+__device__ __forceinline__ float stored_value(const Planes<OPS>& x, size_t o) {
+  if constexpr (OPS == 2) return __half2float(x.hi[o]) + __half2float(x.lo[o]);
+  else return __half2float(x.hi[o]);
+}
+
+// fp32 NCHW planes -> zero-bordered NHWC fp16 hi/lo, or one fp16 (channels padded to cpad)
+template <int OPS>
 __global__ void k_pack_planes(const float* __restrict__ planes, const int* __restrict__ n_dev, int n_max, int F, int H,
-                              int W, int cpad, int guard, int S, float scale, __half* hi, __half* lo) {
+                              int W, int cpad, int guard, int S, float scale, Planes<OPS> out) {
   const int n = min(*n_dev, n_max);
   const int HW = H * W, Wp = W + 1;
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -40,17 +49,17 @@ __global__ void k_pack_planes(const float* __restrict__ planes, const int* __res
   const int hw = (int)((idx / cpad) % HW);
   const int b = (int)(idx / ((size_t)cpad * HW));
   const int y = hw / W, x = hw - y * W;
-  __half h, l;
-  split_hi_lo(plane_input(planes, F, HW, b, c, hw, true, scale), h, l);
+  const float v = plane_input(planes, F, HW, b, c, hw, true, scale);
   const size_t o = ((size_t)guard + (size_t)b * S + y * Wp + x) * cpad + c;
-  hi[o] = h;
-  lo[o] = l;
+  if constexpr (OPS == 2) split_hi_lo(v, out.hi[o], out.lo[o]);
+  else out.hi[o] = __float2half_rn(v);
 }
 // The two 1x1 head convs (K->2 policy, K->1 value; dual.go:70,85) + BN-test affine + ReLU straight
-// from the tower's NHWC hi/lo output: one warp per board point, lanes split the channels
+// from the tower's NHWC hi/lo (or single fp16) output: one warp per board point, lanes split the channels
 // (coalesced 16-byte loads), three dot products reduced with shuffles.
 //   ph [n][2][HW], vh [n][HW]  (the layout the linear layers consume)
-__global__ void k_head_convs_nhwc(const __half* __restrict__ hi, const __half* __restrict__ lo, const int* __restrict__ n_dev,
+template <int OPS>
+__global__ void k_head_convs_nhwc(const Planes<OPS> act, const int* __restrict__ n_dev,
                                   int n_max, int K, int H, int W, int guard, int S, float inv_scale, const float* __restrict__ wp,
                                   const float* __restrict__ gp, const float* __restrict__ bp, const float* __restrict__ wv,
                                   const float* __restrict__ gv, const float* __restrict__ bv, float* ph, float* vh) {
@@ -64,13 +73,16 @@ __global__ void k_head_convs_nhwc(const __half* __restrict__ hi, const __half* _
   const size_t row = (size_t)guard + (size_t)b * S + y * Wp + x;
   float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f;
   for (int c0 = lane * 8; c0 < K; c0 += 256) {
-    const uint4 h4 = *(const uint4*)(hi + row * K + c0);
-    const uint4 l4 = *(const uint4*)(lo + row * K + c0);
+    const uint4 h4 = *(const uint4*)(act.hi + row * K + c0);
+    uint4 l4;
+    if constexpr (OPS == 2) l4 = *(const uint4*)(act.lo + row * K + c0);
     const __half* hh = (const __half*)&h4;
     const __half* ll = (const __half*)&l4;
 #pragma unroll
     for (int i = 0; i < 8; i++) {
-      const float v = (__half2float(hh[i]) + __half2float(ll[i])) * inv_scale;
+      float v;
+      if constexpr (OPS == 2) v = (__half2float(hh[i]) + __half2float(ll[i])) * inv_scale;
+      else v = __half2float(hh[i]) * inv_scale;
       a0 = fmaf(v, __ldg(wp + c0 + i), a0);
       a1 = fmaf(v, __ldg(wp + K + c0 + i), a1);
       a2 = fmaf(v, __ldg(wv + c0 + i), a2);
@@ -92,9 +104,10 @@ __global__ void k_head_convs_nhwc(const __half* __restrict__ hi, const __half* _
     vh[(size_t)b * HW + hw] = v0 > 0.0f ? v0 : 0.0f;
   }
 }
-// diagnostics: the NHWC hi/lo tower output (the values k_head_convs_nhwc reads) -> fp32 NCHW [n][K][HW]
-__global__ void k_tower_nchw(const __half* __restrict__ hi, const __half* __restrict__ lo, const int* __restrict__ n_dev, int n_max,
-                             int K, int H, int W, int guard, int S, float inv_scale, float* out) {
+// diagnostics: the NHWC tower output (the values k_head_convs_nhwc reads) -> fp32 NCHW [n][K][HW]
+template <int OPS>
+__global__ void k_tower_nchw(const Planes<OPS> act, const int* __restrict__ n_dev, int n_max, int K, int H, int W, int guard, int S,
+                             float inv_scale, float* out) {
   const int n = min(*n_dev, n_max);
   const int HW = H * W, Wp = W + 1;
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -102,7 +115,7 @@ __global__ void k_tower_nchw(const __half* __restrict__ hi, const __half* __rest
   const int hw = (int)(idx % HW), c = (int)((idx / HW) % K), b = (int)(idx / ((size_t)HW * K));
   const int y = hw / W, x = hw - y * W;
   const size_t o = ((size_t)guard + (size_t)b * S + y * Wp + x) * K + c;
-  out[idx] = (__half2float(hi[o]) + __half2float(lo[o])) * inv_scale;
+  out[idx] = stored_value<OPS>(act, o) * inv_scale;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -113,46 +126,57 @@ __global__ void k_tower_nchw(const __half* __restrict__ hi, const __half* __rest
 // across layers and samples, one stage per (layer, tap)), and the last layer writes the NHWC hi/lo buffer the head
 // kernels read.  Activations are stored K-major without swizzle ([8-channel chunk][row][16 B]), so tap (dy, dx) is the
 // same tile with its descriptor starting dy*(W+1)+dx rows further — no copy per tap.  Same MMA sequence (tap by tap, three
-// passes), same epilogue arithmetic as the per-layer kernels: the outputs are identical to that path.
+// passes), same epilogue arithmetic as the per-layer kernels: the outputs are identical to that path.  The body is
+// instantiated for both operand forms: k_net_small (hi/lo planes, three passes) and k_smallnet_fp16 (one fp16 plane per
+// operand, one pass, the epilogue of k_conv3x3_tc's single-plane form); the freed shared memory deepens the filter ring.
 constexpr int SN_MAXL = 8;                 // init conv + up to 7 blocks
 constexpr int SN_R0 = 16;                  // halo rows in front of the tile (>= W + 2)
 constexpr int SN_HR = 160;                 // rows per activation plane: halo + 128 + halo
 constexpr int SN_PLANE = 8 * SN_HR * 16;   // one fp16 plane: 8 chunks of 8 channels x SN_HR rows x 16 B
-constexpr int SN_NST = 4;                  // filter stages
-constexpr int SN_STAGE = 2 * 128 * BK * 2; // hi + lo filter tiles of up to 128 rows x 64 K
-__host__ __device__ constexpr int smem_bytes_small() { return 4 * SN_PLANE + SN_NST * SN_STAGE + 1024 + 256; }
-struct SmallMaps { CUtensorMap hi[SN_MAXL], lo[SN_MAXL]; };
+constexpr int SN_TILE = 128 * BK * 2;      // one filter plane of up to 128 rows x 64 K
+// a filter stage holds OPS planes; the ring takes what the two activation buffers leave (4 stages for hi/lo, 11 for fp16)
+__host__ __device__ constexpr int sn_stage_bytes(int OPS) { return OPS * SN_TILE; }
+__host__ __device__ constexpr int sn_stages(int OPS) { return (SMEM_RING_BUDGET - 2 * OPS * SN_PLANE) / sn_stage_bytes(OPS); }
+__host__ __device__ constexpr int smem_bytes_small(int OPS) {
+  return 2 * OPS * SN_PLANE + sn_stages(OPS) * sn_stage_bytes(OPS) + 1024 + 256;
+}
+template <int OPS> struct SmallMaps { PlaneMaps<OPS> w[SN_MAXL]; };
+template <int OPS>
 struct SmallNetArgs {
   const float* planes;  // [n][F][HW] encoder planes
   const int* n_dev;
   int n_max, F, H, W, Wp, S, HW, nlayers, guard;
   float act_scale;
   const float2* aff[SN_MAXL];  // per layer [HW][n_total] {A', B}
-  __half *out_hi, *out_lo;     // last layer: [(guard + n*S)][64], the layout k_head_convs_nhwc reads
+  Planes<OPS> out;             // last layer: [(guard + n*S)][64], the layout k_head_convs_nhwc reads
   int* err;
 };
 
 // one layer of one sample: 9 taps of the filter ring into acc, then the epilogue into smem (or global for the last layer)
-template <int N>
-__device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int smp, uint32_t act, uint32_t stages,
-                                            const MbarRing<SN_NST>& ring, uint32_t& it, int in, bool& overflow) {
+template <int N, int OPS>
+__device__ __forceinline__ void small_layer(const SmallNetArgs<OPS>& a, int l, int smp, uint32_t act, uint32_t stages,
+                                            const MbarRing<sn_stages(OPS)>& ring, uint32_t& it, int in, bool& overflow) {
   constexpr bool PAIR = N == 128;
   constexpr int OUTC = PAIR ? N / 2 : N;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
   int row0, col0;
   acc_frag_origin(warp, lane, row0, col0);
-  const uint32_t in_hi = act + (2 * in) * SN_PLANE, in_lo = in_hi + SN_PLANE;
+  const uint32_t in_hi = act + (OPS * in) * SN_PLANE;
   float acc[N / 2];
   for (int tap = 0; tap < 9; tap++, it++) {
     ring.consumer_wait(it);
     const uint32_t shift = (uint32_t)(SN_R0 + wg * 64 + (tap / 3 - 1) * a.Wp + (tap % 3 - 1)) * 16;
-    const uint32_t sb = stages + ring.stage(it) * SN_STAGE;
-    mma_kblock<N, 0>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_lo + shift, SN_HR * 16),
-                     make_desc_sw(sb), make_desc_sw(sb + SN_STAGE / 2), 32 >> 4, tap == 0, 2 * SN_HR * 16 >> 4);
+    const uint32_t sb = stages + ring.stage(it) * sn_stage_bytes(OPS);
+    if constexpr (OPS == 2)
+      mma_kblock<N, 0>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_hi + SN_PLANE + shift, SN_HR * 16),
+                       make_desc_sw(sb), make_desc_sw(sb + SN_TILE), 32 >> 4, tap == 0, 2 * SN_HR * 16 >> 4);
+    else
+      mma_kblock<N, 0, 1>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), 0, make_desc_sw(sb), 0, 32 >> 4, tap == 0,
+                          2 * SN_HR * 16 >> 4);
     ring.consumer_release(it);
   }
   const bool last = l == a.nlayers - 1;
-  const uint32_t out_hi = act + (2 * (in ^ 1)) * SN_PLANE, out_lo = out_hi + SN_PLANE;
+  const uint32_t out_hi = act + (OPS * (in ^ 1)) * SN_PLANE;
   const int n_total = PAIR ? 128 : 64;
 #pragma unroll
   for (int h = 0; h < 2; h++) {
@@ -167,18 +191,23 @@ __device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int sm
       __half hv[2], lv[2];
 #pragma unroll
       for (int e = 0; e < 2; e++) {
-        split_hi_lo(valid ? fused_value<N, PAIR>(aff, acc, j, h, e, a.act_scale) : 0.0f, hv[e], lv[e]);
+        const float v = valid ? fused_value<N, PAIR>(aff, acc, j, h, e, a.act_scale) : 0.0f;
+        if constexpr (OPS == 2) split_hi_lo(v, hv[e], lv[e]);
+        else hv[e] = __float2half_rn(v);
         overflow |= !(fabsf(__half2float(hv[e])) <= 65504.0f);
       }
       const int c = 8 * j + col0;
       if (last) {
-        *reinterpret_cast<__half2*>(a.out_hi + grow * 64 + c) = __halves2half2(hv[0], hv[1]);
-        *reinterpret_cast<__half2*>(a.out_lo + grow * 64 + c) = __halves2half2(lv[0], lv[1]);
+        *reinterpret_cast<__half2*>(a.out.hi + grow * 64 + c) = __halves2half2(hv[0], hv[1]);
+        if constexpr (OPS == 2) *reinterpret_cast<__half2*>(a.out.lo + grow * 64 + c) = __halves2half2(lv[0], lv[1]);
       } else {  // chunk c / 8, row SN_R0 + p, byte (c % 8) * 2; invalid positions are written as zeros
         const uint32_t o = (uint32_t)(c >> 3) * (SN_HR * 16) + (uint32_t)(SN_R0 + p) * 16 + (uint32_t)(c & 7) * 2;
-        const __half2 h2 = __halves2half2(hv[0], hv[1]), l2 = __halves2half2(lv[0], lv[1]);
+        const __half2 h2 = __halves2half2(hv[0], hv[1]);
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_hi + o), "r"(*reinterpret_cast<const uint32_t*>(&h2)) : "memory");
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_lo + o), "r"(*reinterpret_cast<const uint32_t*>(&l2)) : "memory");
+        if constexpr (OPS == 2) {
+          const __half2 l2 = __halves2half2(lv[0], lv[1]);
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(out_hi + SN_PLANE + o), "r"(*reinterpret_cast<const uint32_t*>(&l2)) : "memory");
+        }
       }
     }
   }
@@ -187,15 +216,17 @@ __device__ __forceinline__ void small_layer(const SmallNetArgs& a, int l, int sm
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 __device__ __forceinline__ void proxy_fence() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-__global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant__ SmallMaps maps, SmallNetArgs a) {
+template <int OPS>
+__device__ __forceinline__ void net_small(const SmallMaps<OPS>& maps, const SmallNetArgs<OPS>& a) {
+  constexpr int NST = sn_stages(OPS);
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-  const uint32_t act = base;                       // 4 planes: buffer b hi at 2b, lo at 2b + 1
-  const uint32_t stages = base + 4 * SN_PLANE;      // filter stages (1024-aligned: SN_PLANE is a multiple of 1024)
-  const MbarRing<SN_NST> ring{stages + SN_NST * SN_STAGE};
+  const uint32_t act = base;                         // 2 * OPS planes: buffer b hi at OPS*b, lo (OPS = 2) at 2b + 1
+  const uint32_t stages = base + 2 * OPS * SN_PLANE;  // filter stages (1024-aligned: SN_PLANE is a multiple of 1024)
+  const MbarRing<NST> ring{stages + NST * sn_stage_bytes(OPS)};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int i = threadIdx.x; i < 4 * SN_PLANE / 16; i += blockDim.x) reinterpret_cast<uint4*>(base_ptr)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = threadIdx.x; i < 2 * OPS * SN_PLANE / 16; i += blockDim.x) reinterpret_cast<uint4*>(base_ptr)[i] = make_uint4(0, 0, 0, 0);
   ring.init(CONSUMER_WARPS);
   proxy_fence();  // the zeroed halo rows are read by wgmma
   __syncthreads();
@@ -205,12 +236,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
       uint32_t it = 0;
       for (int smp = blockIdx.x; smp < n; smp += gridDim.x)
         for (int l = 0; l < a.nlayers; l++) {
-          const uint32_t bytes = 2u * (l == 0 ? 64 : 128) * BK * 2;
+          const uint32_t bytes = OPS * (l == 0 ? 64 : 128) * BK * 2;
           for (int tap = 0; tap < 9; tap++, it++) {
             ring.producer_acquire(it, bytes);
-            const uint32_t sb = stages + ring.stage(it) * SN_STAGE;
-            tma_load_2d(sb, &maps.hi[l], ring.full(it), tap * BK, 0);
-            tma_load_2d(sb + SN_STAGE / 2, &maps.lo[l], ring.full(it), tap * BK, 0);
+            const uint32_t sb = stages + ring.stage(it) * sn_stage_bytes(OPS);
+            tma_load_2d(sb, &maps.w[l].hi, ring.full(it), tap * BK, 0);
+            if constexpr (OPS == 2) tma_load_2d(sb + SN_TILE, &maps.w[l].lo, ring.full(it), tap * BK, 0);
           }
         }
     }
@@ -226,18 +257,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant
       const int y = p / a.Wp, x = p - y * a.Wp;
       const float v = plane_input(a.planes, a.F, a.HW, smp, c, y * a.W + x, p < a.S && y < a.H && x < a.W, a.act_scale);
       const uint32_t o = (uint32_t)(c >> 3) * (SN_HR * 16) + (uint32_t)(SN_R0 + p) * 16 + (uint32_t)(c & 7) * 2;
-      split_hi_lo(v, *reinterpret_cast<__half*>(base_ptr + o), *reinterpret_cast<__half*>(base_ptr + SN_PLANE + o));
+      if constexpr (OPS == 2) split_hi_lo(v, *reinterpret_cast<__half*>(base_ptr + o), *reinterpret_cast<__half*>(base_ptr + SN_PLANE + o));
+      else *reinterpret_cast<__half*>(base_ptr + o) = __float2half_rn(v);
     }
     proxy_fence();
     consumer_sync();
     for (int l = 0; l < a.nlayers; l++) {
-      if (l == 0) small_layer<64>(a, l, smp, act, stages, ring, it, 0, overflow);
-      else small_layer<128>(a, l, smp, act, stages, ring, it, l & 1, overflow);
+      if (l == 0) small_layer<64, OPS>(a, l, smp, act, stages, ring, it, 0, overflow);
+      else small_layer<128, OPS>(a, l, smp, act, stages, ring, it, l & 1, overflow);
       proxy_fence();   // this layer's generic smem writes are read by the next layer's wgmma (async proxy)
       consumer_sync(); // and every warp's MMAs on the buffer the next layer overwrites have completed
     }
   }
   if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
+}
+__global__ void __launch_bounds__(NTHREADS, 1) k_net_small(const __grid_constant__ SmallMaps<2> maps, SmallNetArgs<2> a) {
+  net_small<2>(maps, a);
+}
+__global__ void __launch_bounds__(NTHREADS, 1) k_smallnet_fp16(const __grid_constant__ SmallMaps<1> maps, SmallNetArgs<1> a) {
+  net_small<1>(maps, a);
 }
 
 // dynamic shared memory opt-in of every instantiation this file launches, on the current device (called from the
@@ -246,20 +284,24 @@ void tower_configure_device() {
   set_conv_attr<256, true>(); set_conv_attr<128, true>(); set_conv_attr<256, false>(); set_conv_attr<128, false>();
   set_conv_attr<64, false>();
   set_conv_attr<256, true, 1>(); set_conv_attr<256, true, 2>(); set_conv_attr<128, true, 1>(); set_conv_attr<128, true, 2>();
-  CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small()));
+  set_conv_attr<256, true, 1, 1>(); set_conv_attr<128, true, 1, 1>(); set_conv_attr<256, false, 1, 1>();
+  set_conv_attr<128, false, 1, 1>(); set_conv_attr<64, false, 1, 1>();
+  CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small(2)));
+  CUDA_CHECK(cudaFuncSetAttribute(k_smallnet_fp16, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small(1)));
 }
 
 struct Layer {
   int cin, n_total, bn;
   bool pair;
-  __half *w_hi = nullptr, *w_lo = nullptr;  // [n_total][9*cin]
+  __half *w_hi = nullptr, *w_lo = nullptr;  // [n_total][9*cin]; no w_lo in fp16 mode
   float2* aff = nullptr;                    // [HW][n_total] {A', B} in weight-row order
   CUtensorMap mB_hi, mB_lo;
 };
 struct Impl {
   NetDims d;
   int n_max, ea, guard, S, rows_alloc, num_sms, passes = TC_PASSES, mode3d = 0, tps = 1;
-  bool small = false;  // K = 64, (H+1)(W+1) <= 128: the whole tower of a sample in one kernel (k_net_small)
+  bool fp16 = false;   // AZ_FLAG_FP16_TOWER: one fp16 plane per operand (no *_lo buffers or maps), one pass
+  bool small = false;  // K = 64, (H+1)(W+1) <= 128: the whole tower of a sample in one kernel (k_net_small / k_smallnet_fp16)
   __half *xin_hi = nullptr, *xin_lo = nullptr;  // [(guard+rows+guard)][64]
   __half *x_hi[2] = {nullptr, nullptr}, *x_lo[2] = {nullptr, nullptr};  // [(guard+rows+guard)][K]
   CUtensorMap mIn_hi, mIn_lo, mX_hi[2], mX_lo[2];
@@ -276,28 +318,49 @@ struct Impl {
   }
 };
 
+// the host's view of one operand in the kernels' form: hi and lo, or hi alone (lo is not allocated in fp16 mode)
+template <int OPS> Planes<OPS> planes_of(__half* hi, __half* lo) {
+  if constexpr (OPS == 2) return {hi, lo};
+  else return {hi};
+}
+template <int OPS> PlaneMaps<OPS> maps_of(const CUtensorMap& hi, const CUtensorMap& lo) {
+  if constexpr (OPS == 2) return {hi, lo};
+  else return {hi};
+}
+
 // AZ_TC_PASSES (diagnostics) selects 1 or 2 passes for the fused layers; the other shapes always run three
 template <int BN>
-void launch_fused(int passes, const CUtensorMap& ah, const CUtensorMap& al, const Layer& L, const ConvArgs& a, int num_sms,
+void launch_fused(int passes, const PlaneMaps<2>& A, const PlaneMaps<2>& B, const ConvArgs& a, const Planes<2>& out, int num_sms,
                   cudaStream_t st) {
-  if (passes == 1) launch_conv<BN, true, 1>(ah, al, L.mB_hi, L.mB_lo, a, num_sms, st);
-  else if (passes == 2) launch_conv<BN, true, 2>(ah, al, L.mB_hi, L.mB_lo, a, num_sms, st);
-  else launch_conv<BN, true>(ah, al, L.mB_hi, L.mB_lo, a, num_sms, st);
+  if (passes == 1) launch_conv<BN, true, 1>(A, B, a, out, num_sms, st);
+  else if (passes == 2) launch_conv<BN, true, 2>(A, B, a, out, num_sms, st);
+  else launch_conv<BN, true>(A, B, a, out, num_sms, st);
 }
-void dispatch_conv(const Impl& I, const Layer& L, const CUtensorMap& ah, const CUtensorMap& al, __half* ohi, __half* olo,
-                   const int* n_dev, int* err, cudaStream_t st) {
+template <int OPS>
+void dispatch_conv(const Impl& I, const Layer& L, const PlaneMaps<OPS>& A, const Planes<OPS>& out, const int* n_dev, int* err,
+                   cudaStream_t st) {
   ConvArgs a;
   a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
   a.mode3d = I.mode3d; a.tps = I.tps;
-  a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff; a.out_hi = ohi; a.out_lo = olo;
+  a.cin = L.cin; a.n_total = L.n_total; a.cout = I.d.K; a.aff = L.aff;
   a.act_scale = ldexpf(1.0f, I.ea); a.err = err;
   a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
-  if (L.pair && L.bn == 256) launch_fused<256>(I.passes, ah, al, L, a, I.num_sms, st);
-  else if (L.pair && L.bn == 128) launch_fused<128>(I.passes, ah, al, L, a, I.num_sms, st);
-  else if (!L.pair && L.bn == 256) launch_conv<256, false>(ah, al, L.mB_hi, L.mB_lo, a, I.num_sms, st);
-  else if (!L.pair && L.bn == 128) launch_conv<128, false>(ah, al, L.mB_hi, L.mB_lo, a, I.num_sms, st);
-  else if (!L.pair && L.bn == 64) launch_conv<64, false>(ah, al, L.mB_hi, L.mB_lo, a, I.num_sms, st);
-  else throw std::runtime_error("tc tower: unsupported tile");
+  const PlaneMaps<OPS> B = maps_of<OPS>(L.mB_hi, L.mB_lo);
+  if constexpr (OPS == 1) {  // one pass whatever AZ_TC_PASSES says
+    if (L.pair && L.bn == 256) launch_conv<256, true, 1, 1>(A, B, a, out, I.num_sms, st);
+    else if (L.pair && L.bn == 128) launch_conv<128, true, 1, 1>(A, B, a, out, I.num_sms, st);
+    else if (!L.pair && L.bn == 256) launch_conv<256, false, 1, 1>(A, B, a, out, I.num_sms, st);
+    else if (!L.pair && L.bn == 128) launch_conv<128, false, 1, 1>(A, B, a, out, I.num_sms, st);
+    else if (!L.pair && L.bn == 64) launch_conv<64, false, 1, 1>(A, B, a, out, I.num_sms, st);
+    else throw std::runtime_error("tc tower: unsupported tile");
+  } else {
+    if (L.pair && L.bn == 256) launch_fused<256>(I.passes, A, B, a, out, I.num_sms, st);
+    else if (L.pair && L.bn == 128) launch_fused<128>(I.passes, A, B, a, out, I.num_sms, st);
+    else if (!L.pair && L.bn == 256) launch_conv<256, false>(A, B, a, out, I.num_sms, st);
+    else if (!L.pair && L.bn == 128) launch_conv<128, false>(A, B, a, out, I.num_sms, st);
+    else if (!L.pair && L.bn == 64) launch_conv<64, false>(A, B, a, out, I.num_sms, st);
+    else throw std::runtime_error("tc tower: unsupported tile");
+  }
 }
 
 }  // namespace
@@ -307,11 +370,11 @@ bool tc_tower_supported(const NetDims& d) {
   return (d.K == 64 || d.K == 128 || d.K == 256) && d.F <= 64 && d.SharedLayers >= 0;
 }
 
-void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2) {
+void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2, bool fp16) {
   tower_configure_device();
   Impl* I = new Impl;
   t.impl = I;
-  I->d = d; I->n_max = n_max; I->ea = act_scale_log2;
+  I->d = d; I->n_max = n_max; I->ea = act_scale_log2; I->fp16 = fp16;
   if (const char* ps = getenv("AZ_TC_PASSES")) { int v = atoi(ps); if (v >= 1 && v <= 3) I->passes = v; }  // experiments only
   // layout choice by padded-row overhead (rows computed per real board point)
   const int S_flat = (d.H + 1) * (d.W + 1), S_ps = d.H * (d.W + 1), tps = (S_ps + BM - 1) / BM;
@@ -322,14 +385,16 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2)
   CUDA_CHECK(cudaGetDevice(&dev));
   CUDA_CHECK(cudaDeviceGetAttribute(&I->num_sms, cudaDevAttrMultiProcessorCount, dev));
   auto alloc_h = [&](size_t n) { __half* p; CUDA_CHECK(cudaMalloc(&p, n * 2)); CUDA_CHECK(cudaMemset(p, 0, n * 2)); return p; };
-  I->xin_hi = alloc_h((size_t)I->rows_alloc * 64); I->xin_lo = alloc_h((size_t)I->rows_alloc * 64);
-  for (int i = 0; i < 2; i++) { I->x_hi[i] = alloc_h((size_t)I->rows_alloc * d.K); I->x_lo[i] = alloc_h((size_t)I->rows_alloc * d.K); }
-  if (I->mode3d) {
-    I->mIn_hi = make_map3d(I->xin_hi, n_max, I->S, 64); I->mIn_lo = make_map3d(I->xin_lo, n_max, I->S, 64);
-    for (int i = 0; i < 2; i++) { I->mX_hi[i] = make_map3d(I->x_hi[i], n_max, I->S, d.K); I->mX_lo[i] = make_map3d(I->x_lo[i], n_max, I->S, d.K); }
-  } else {
-    I->mIn_hi = make_map(I->xin_hi, I->rows_alloc, 64, BM); I->mIn_lo = make_map(I->xin_lo, I->rows_alloc, 64, BM);
-    for (int i = 0; i < 2; i++) { I->mX_hi[i] = make_map(I->x_hi[i], I->rows_alloc, d.K, BM); I->mX_lo[i] = make_map(I->x_lo[i], I->rows_alloc, d.K, BM); }
+  // an activation buffer [(guard+rows+guard)][cols] and its tensor map; the lo planes exist only in the hi/lo form
+  auto act_buf = [&](int cols, __half*& p, CUtensorMap& m) {
+    p = alloc_h((size_t)I->rows_alloc * cols);
+    m = I->mode3d ? make_map3d(p, n_max, I->S, cols) : make_map(p, I->rows_alloc, cols, BM);
+  };
+  act_buf(64, I->xin_hi, I->mIn_hi);
+  if (!fp16) act_buf(64, I->xin_lo, I->mIn_lo);
+  for (int i = 0; i < 2; i++) {
+    act_buf(d.K, I->x_hi[i], I->mX_hi[i]);
+    if (!fp16) act_buf(d.K, I->x_lo[i], I->mX_lo[i]);
   }
   // layers: init (single), then SharedLayers fused pairs
   const int K = d.K, HW = d.HW();
@@ -340,9 +405,10 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2)
     L.n_total = L.pair ? 2 * K : K;
     L.bn = std::min(256, L.n_total);
     const size_t ktot = (size_t)9 * L.cin;
-    L.w_hi = alloc_h((size_t)L.n_total * ktot); L.w_lo = alloc_h((size_t)L.n_total * ktot);
+    L.w_hi = alloc_h((size_t)L.n_total * ktot);
+    L.mB_hi = make_map(L.w_hi, L.n_total, ktot, L.bn);
+    if (!fp16) { L.w_lo = alloc_h((size_t)L.n_total * ktot); L.mB_lo = make_map(L.w_lo, L.n_total, ktot, L.bn); }
     CUDA_CHECK(cudaMalloc(&L.aff, (size_t)HW * L.n_total * sizeof(float2)));
-    L.mB_hi = make_map(L.w_hi, L.n_total, ktot, L.bn); L.mB_lo = make_map(L.w_lo, L.n_total, ktot, L.bn);
     I->layers.push_back(L);
   }
   I->small = d.K == 64 && !I->mode3d && I->S <= BM && d.W + 2 <= SN_R0 && (int)I->layers.size() <= SN_MAXL && d.F <= 64;
@@ -353,6 +419,7 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2)
 int tc_tower_kernel_kind(const TcTower& t) {
   const Impl* I = (const Impl*)t.impl;
   if (!I) return -1;
+  if (I->fp16) return I->small ? 7 : 6;
   return I->small ? 5 : 0;
 }
 
@@ -368,7 +435,7 @@ void tc_tower_free(TcTower& t) {
 }
 
 // Host-side operand preparation (once per Agent.SwitchToInference): split the fp32 filters into
-// fp16 hi/lo at a per-layer power-of-two scale, reorder rows so that an N tile holds the same
+// fp16 hi/lo (fp16 mode: round them to one fp16) at a per-layer power-of-two scale, reorder rows so that an N tile holds the same
 // output channels of both branches, fold BN-test (x/sqrt(eps)), gamma and the scales into A'.
 void tc_tower_prepare(TcTower& t, const Snapshot& s, cudaStream_t st) {
   Impl* I = (Impl*)t.impl;
@@ -392,7 +459,7 @@ void tc_tower_prepare(TcTower& t, const Snapshot& s, cudaStream_t st) {
     int ew = 0;
     if (mx > 0 && std::isfinite(mx)) { int e2; frexpf(mx, &e2); ew = 7 - e2; }  // mx*2^ew in [64,128)
     const float wscale = ldexpf(1.0f, ew);
-    std::vector<__half> whi((size_t)L.n_total * ktot, __float2half_rn(0.0f)), wlo((size_t)L.n_total * ktot, __float2half_rn(0.0f));
+    std::vector<__half> whi((size_t)L.n_total * ktot, __float2half_rn(0.0f)), wlo(I->fp16 ? 0 : whi.size(), __float2half_rn(0.0f));
     std::vector<float2> aff((size_t)HW * L.n_total);
     const int half_bn = L.pair ? L.bn / 2 : L.bn;
     const float fold = ldexpf(1.0f, -(I->ea + ew)) * inv_sd;
@@ -404,54 +471,59 @@ void tc_tower_prepare(TcTower& t, const Snapshot& s, cudaStream_t st) {
       for (int tap = 0; tap < 9; tap++)
         for (int ci = 0; ci < ci_real; ci++) {
           const size_t o = (size_t)row * ktot + (size_t)tap * L.cin + ci;
-          split_hi_lo(f[ci * 9 + tap] * wscale, whi[o], wlo[o]);  // filter[co][ci][ky][kx], tap = ky*3+kx
+          const float w = f[ci * 9 + tap] * wscale;  // filter[co][ci][ky][kx], tap = ky*3+kx
+          if (I->fp16) whi[o] = __float2half_rn(w);
+          else split_hi_lo(w, whi[o], wlo[o]);
         }
       const float* g = h.data() + u[br]->gamma + (size_t)ch * HW;
       const float* be = h.data() + u[br]->beta + (size_t)ch * HW;
       for (int hw = 0; hw < HW; hw++) aff[(size_t)hw * L.n_total + row] = make_float2(g[hw] * fold, be[hw]);
     }
     CUDA_CHECK(cudaMemcpy(L.w_hi, whi.data(), whi.size() * 2, cudaMemcpyHostToDevice));
-    CUDA_CHECK(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
+    if (!I->fp16) CUDA_CHECK(cudaMemcpy(L.w_lo, wlo.data(), wlo.size() * 2, cudaMemcpyHostToDevice));
     CUDA_CHECK(cudaMemcpy(L.aff, aff.data(), aff.size() * sizeof(float2), cudaMemcpyHostToDevice));
   }
   t.ready = true;
 }
 
-void tc_tower_forward(TcTower& t, const NetLayout& NL, const Snapshot& s, Fp32Scratch& sc, const float* planes,
-                      const int* n_dev, int n_max, float* policy, int ldp, float* value, int* err_flag, cudaStream_t st,
-                      unsigned long long* launches) {
-  Impl* I = (Impl*)t.impl;
-  if (!I || !t.ready) throw std::runtime_error("tc tower not prepared");
+template <int OPS>
+void tower_forward(Impl* I, const NetLayout& NL, const Snapshot& s, Fp32Scratch& sc, const float* planes, const int* n_dev,
+                   int n_max, float* policy, int ldp, float* value, int* err_flag, cudaStream_t st, unsigned long long* launches) {
   const NetDims& d = I->d;
   const float scale = ldexpf(1.0f, I->ea);
   const size_t f0 = I->profile ? I->ev_get(st) : 0;
   int cur = 0;
-  if (I->small) {  // every conv layer of every leaf in one launch; the head kernels read its output from x_hi[0] / x_lo[0]
-    SmallMaps maps;
-    SmallNetArgs a;
+  if (I->small) {  // every conv layer of every leaf in one launch; the head kernels read its output from buffer 0
+    SmallMaps<OPS> maps;
+    SmallNetArgs<OPS> a;
     a.planes = planes; a.n_dev = n_dev; a.n_max = n_max; a.F = d.F; a.H = d.H; a.W = d.W; a.Wp = d.W + 1; a.S = I->S;
     a.HW = d.HW(); a.nlayers = (int)I->layers.size(); a.guard = I->guard; a.act_scale = scale;
     for (int l = 0; l < SN_MAXL; l++) {
       const Layer& Lr = I->layers[std::min<size_t>(l, I->layers.size() - 1)];
-      maps.hi[l] = Lr.mB_hi; maps.lo[l] = Lr.mB_lo; a.aff[l] = Lr.aff;
+      maps.w[l] = maps_of<OPS>(Lr.mB_hi, Lr.mB_lo); a.aff[l] = Lr.aff;
     }
-    a.out_hi = I->x_hi[0]; a.out_lo = I->x_lo[0]; a.err = err_flag;
+    a.out = planes_of<OPS>(I->x_hi[0], I->x_lo[0]); a.err = err_flag;
     const size_t e0 = I->profile ? I->ev_get(st) : 0;
-    k_net_small<<<std::max(1, std::min(n_max, I->num_sms)), NTHREADS, smem_bytes_small(), st>>>(maps, a); LAUNCH_CHECK();
+    const int grid = std::max(1, std::min(n_max, I->num_sms));
+    if constexpr (OPS == 2) k_net_small<<<grid, NTHREADS, smem_bytes_small(OPS), st>>>(maps, a);
+    else k_smallnet_fp16<<<grid, NTHREADS, smem_bytes_small(OPS), st>>>(maps, a);
+    LAUNCH_CHECK();
     if (I->profile) I->conv_spans.push_back({e0, I->ev_get(st)});
     if (launches) (*launches)++;
   } else {
   {
     size_t total = (size_t)n_max * d.HW() * 64;
-    k_pack_planes<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(planes, n_dev, n_max, d.F, d.H, d.W, 64, I->guard, I->S, scale,
-                                                                  I->xin_hi, I->xin_lo); LAUNCH_CHECK();
+    k_pack_planes<OPS><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(planes, n_dev, n_max, d.F, d.H, d.W, 64, I->guard, I->S,
+                                                                       scale, planes_of<OPS>(I->xin_hi, I->xin_lo)); LAUNCH_CHECK();
     if (launches) (*launches)++;
   }
-  dispatch_conv(*I, I->layers[0], I->mIn_hi, I->mIn_lo, I->x_hi[0], I->x_lo[0], n_dev, err_flag, st);
+  dispatch_conv<OPS>(*I, I->layers[0], maps_of<OPS>(I->mIn_hi, I->mIn_lo), planes_of<OPS>(I->x_hi[0], I->x_lo[0]), n_dev, err_flag,
+                     st);
   if (launches) (*launches)++;
   for (size_t l = 1; l < I->layers.size(); l++) {
     size_t e0 = I->profile ? I->ev_get(st) : 0;
-    dispatch_conv(*I, I->layers[l], I->mX_hi[cur], I->mX_lo[cur], I->x_hi[cur ^ 1], I->x_lo[cur ^ 1], n_dev, err_flag, st);
+    dispatch_conv<OPS>(*I, I->layers[l], maps_of<OPS>(I->mX_hi[cur], I->mX_lo[cur]),
+                       planes_of<OPS>(I->x_hi[cur ^ 1], I->x_lo[cur ^ 1]), n_dev, err_flag, st);
     if (I->profile) I->conv_spans.push_back({e0, I->ev_get(st)});
     if (launches) (*launches)++;
     cur ^= 1;
@@ -461,13 +533,22 @@ void tc_tower_forward(TcTower& t, const NetLayout& NL, const Snapshot& s, Fp32Sc
     const SnapUnit& pu = s.units[1 + 2 * d.SharedLayers];
     const SnapUnit& vu = s.units[2 + 2 * d.SharedLayers];
     size_t warps = (size_t)n_max * d.HW();
-    k_head_convs_nhwc<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(
-        I->x_hi[cur], I->x_lo[cur], n_dev, n_max, d.K, d.H, d.W, I->guard, I->S, 1.0f / scale, s.d + pu.filter, s.d + pu.gamma,
-        s.d + pu.beta, s.d + vu.filter, s.d + vu.gamma, s.d + vu.beta, sc.ph, sc.vh); LAUNCH_CHECK();
+    k_head_convs_nhwc<OPS><<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(
+        planes_of<OPS>(I->x_hi[cur], I->x_lo[cur]), n_dev, n_max, d.K, d.H, d.W, I->guard, I->S, 1.0f / scale, s.d + pu.filter,
+        s.d + pu.gamma, s.d + pu.beta, s.d + vu.filter, s.d + vu.gamma, s.d + vu.beta, sc.ph, sc.vh); LAUNCH_CHECK();
     if (launches) (*launches)++;
   }
   heads_tiled(NL, s, sc.ph, sc.vh, n_dev, n_max, policy, ldp, value, st, launches);
   if (I->profile) I->fwd_spans.push_back({f0, I->ev_get(st)});
+}
+
+void tc_tower_forward(TcTower& t, const NetLayout& NL, const Snapshot& s, Fp32Scratch& sc, const float* planes,
+                      const int* n_dev, int n_max, float* policy, int ldp, float* value, int* err_flag, cudaStream_t st,
+                      unsigned long long* launches) {
+  Impl* I = (Impl*)t.impl;
+  if (!I || !t.ready) throw std::runtime_error("tc tower not prepared");
+  if (I->fp16) tower_forward<1>(I, NL, s, sc, planes, n_dev, n_max, policy, ldp, value, err_flag, st, launches);
+  else tower_forward<2>(I, NL, s, sc, planes, n_dev, n_max, policy, ldp, value, err_flag, st, launches);
 }
 
 void tc_tower_output(TcTower& t, const int* n_dev, int n_max, float* out, cudaStream_t st) {
@@ -477,8 +558,15 @@ void tc_tower_output(TcTower& t, const int* n_dev, int n_max, float* out, cudaSt
   // k_net_small leaves the last layer in buffer 0; the per-layer path swaps buffers once per fused layer
   const int last = I->small ? 0 : (int)(I->layers.size() - 1) & 1;
   const size_t total = (size_t)n_max * d.K * d.HW();
-  k_tower_nchw<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(I->x_hi[last], I->x_lo[last], n_dev, n_max, d.K, d.H, d.W, I->guard,
-                                                                I->S, ldexpf(1.0f, -I->ea), out); LAUNCH_CHECK();
+  const unsigned blocks = (unsigned)((total + 255) / 256);
+  const float inv_scale = ldexpf(1.0f, -I->ea);
+  if (I->fp16)
+    k_tower_nchw<1><<<blocks, 256, 0, st>>>(planes_of<1>(I->x_hi[last], nullptr), n_dev, n_max, d.K, d.H, d.W, I->guard, I->S,
+                                            inv_scale, out);
+  else
+    k_tower_nchw<2><<<blocks, 256, 0, st>>>(planes_of<2>(I->x_hi[last], I->x_lo[last]), n_dev, n_max, d.K, d.H, d.W, I->guard, I->S,
+                                            inv_scale, out);
+  LAUNCH_CHECK();
 }
 
 void tc_tower_profile(TcTower& t, bool enable) {

@@ -9,9 +9,10 @@ struct TcTower {
 // shapes the tensor-core tower handles (K multiple of 64, board fits the padded tiling); smaller
 // nets (tic-tac-toe K=3, Connect-4 K=16) run on the fp32 CUDA-core kernels.
 bool tc_tower_supported(const NetDims& d);
-void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2);
+// fp16: AZ_FLAG_FP16_TOWER — activations and filters stored as one fp16 each, one wgmma pass (no lo buffers are allocated)
+void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2, bool fp16);
 // which kernel runs the fused layers (bench labels): 0 = k_conv3x3_tc (wgmma, 3 x fp16), 5 = k_net_small (the whole tower
-// of a K = 64 net in one kernel); -1 = no tensor-core tower
+// of a K = 64 net in one kernel), 6 = k_conv3x3_tc single fp16 plane, 7 = k_smallnet_fp16; -1 = no tensor-core tower
 int tc_tower_kernel_kind(const TcTower& t);
 void tc_tower_free(TcTower& t);
 // split/scale/reorder the snapshot's filters and BN affines into the tensor-core operand layout

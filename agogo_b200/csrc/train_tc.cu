@@ -319,15 +319,16 @@ void tc_gemm_conv(TcGemm& g, const float* x, int Cin, const float* filter, int f
   }
   const int bn = std::min(256, Cout);
   // tensor maps over the (re-used) operand buffers for this shape
-  CUtensorMap mAh = make_map(sl.hi, I->rows_alloc, cpad, BM), mAl = make_map(sl.lo, I->rows_alloc, cpad, BM);
-  CUtensorMap mBh = make_map(I->w_hi, Cout, (uint64_t)9 * cpad, bn), mBl = make_map(I->w_lo, Cout, (uint64_t)9 * cpad, bn);
+  const PlaneMaps<2> mA{make_map(sl.hi, I->rows_alloc, cpad, BM), make_map(sl.lo, I->rows_alloc, cpad, BM)};
+  const PlaneMaps<2> mB{make_map(I->w_hi, Cout, (uint64_t)9 * cpad, bn), make_map(I->w_lo, Cout, (uint64_t)9 * cpad, bn)};
   ConvArgs a;
   a.n_dev = I->dB; a.n_max = I->B; a.S = I->S; a.Wp = d.W + 1; a.H = d.H; a.W = d.W; a.guard = I->guard; a.mode3d = 0; a.tps = 1;
-  a.cin = cpad; a.n_total = Cout; a.cout = Cout; a.aff = nullptr; a.out_hi = nullptr; a.out_lo = nullptr; a.act_scale = 1.0f;
+  a.cin = cpad; a.n_total = Cout; a.cout = Cout; a.aff = nullptr; a.act_scale = 1.0f;
   a.err = nullptr; a.out_raw = I->raw; a.exp_a = sl.exp; a.exp_b = I->exp_b;
-  if (bn == 256) launch_conv<256, false>(mAh, mAl, mBh, mBl, a, I->num_sms, st);
-  else if (bn == 128) launch_conv<128, false>(mAh, mAl, mBh, mBl, a, I->num_sms, st);
-  else launch_conv<64, false>(mAh, mAl, mBh, mBl, a, I->num_sms, st);
+  const Planes<2> none{nullptr, nullptr};  // raw mode: the epilogue writes out_raw
+  if (bn == 256) launch_conv<256, false>(mA, mB, a, none, I->num_sms, st);
+  else if (bn == 128) launch_conv<128, false>(mA, mB, a, none, I->num_sms, st);
+  else launch_conv<64, false>(mA, mB, a, none, I->num_sms, st);
   k_unpack_nchw<<<dim3((HW + 31) / 32, (Cout + 31) / 32, I->B), 256, 0, st>>>(I->raw, I->B, Cout, d.H, d.W, Cout, I->guard, I->S, out, accumulate ? 1 : 0); LAUNCH_CHECK();
   if (launches) *launches += nl + 4;
 }

@@ -110,6 +110,15 @@ typedef struct az_dual_config {
  * only) and Ended adds komi to White.  Same arithmetic everywhere else; engine and oracle are compared bit for bit under
  * the flag too. */
 #define AZ_FLAG_WQ_COMPLETE 8u
+/* fp16 inference tower, a looser result contract than the default: activations (scaled by 2^act_scale_log2) and
+ * filters (scaled by their per-layer power of two) are stored as a single fp16 each; one fp16 wgmma pass per MAC, fp32
+ * accumulation, the same fp32 epilogue and heads.  Per conv layer |dev - ref| <= 2 * 2^-11 * (mag + |ref|) +
+ * 2^-(25 + act_scale_log2), mag = sum |A'| * (|W| (*) |x|) (DESIGN.md section 4).  Applies to every inference of the
+ * tensor-core tower: az_infer, az_infer_tower, and the arena / search evaluations inside the captured wave graph.  Does
+ * not affect training: az_train and az_train_grads keep the three-pass GEMMs.  AZ_FLAG_FP32_TOWER wins over it; it wins
+ * over AZ_FLAG_FAST_TOWER; it is ignored where the tensor-core tower does not apply (K not in {64, 128, 256}).  The CPU
+ * oracle accepts and ignores it, as it ignores the other tower flags. */
+#define AZ_FLAG_FP16_TOWER 16u
 
 typedef struct az_engine_desc {
   az_game_desc game;
@@ -277,7 +286,8 @@ int az_counters_reset(az_engine* e);
  * measurement, enable=0 stops; out (may be NULL) receives {conv_ms_total, conv_launches,
  * forward_ms_total, forward_calls, region_ms, kernel_kind, 0...} accumulated since the last enable=1; region_ms is the
  * device time between the enable=1 and the enable=0 call on the engine's stream; kernel_kind names the kernel that runs
- * the fused layers (0 k_conv3x3_tc, wgmma, three fp16 passes; 5 k_net_small; -1 fp32 tower).  enable=2 times the region only (region_ms): no per-launch events, so
+ * the fused layers (0 k_conv3x3_tc, wgmma, three fp16 passes; 5 k_net_small; 6 k_conv3x3_tc per layer in fp16, one pass
+ * (AZ_FLAG_FP16_TOWER); 7 the fp16 small-net kernel k_smallnet_fp16; -1 fp32 tower; 1-4 were B200 kernels and are not used).  enable=2 times the region only (region_ms): no per-launch events, so
  * the captured wave graph keeps running — what a launch-bound small-net workload should be timed with. */
 int az_profile(az_engine* e, int32_t enable, double out[8]);
 
