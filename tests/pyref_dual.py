@@ -47,8 +47,8 @@ def conv_bwd(x, w, dz):
     dxp = np.zeros_like(xp)
     for ky in range(k):
         for kx in range(k):
-            dw[:, :, ky, kx] = np.einsum("bohw,bchw->oc", dz, xp[:, :, ky:ky + H, kx:kx + W])
-            dxp[:, :, ky:ky + H, kx:kx + W] += np.einsum("oc,bohw->bchw", w[:, :, ky, kx], dz)
+            dw[:, :, ky, kx] = np.tensordot(dz, xp[:, :, ky:ky + H, kx:kx + W], axes=((0, 2, 3), (0, 2, 3)))
+            dxp[:, :, ky:ky + H, kx:kx + W] += np.tensordot(w[:, :, ky, kx], dz, axes=(0, 1)).transpose(1, 0, 2, 3)
     return dw, dxp[:, :, p:p + H, p:p + W]
 
 
@@ -56,12 +56,18 @@ class Unit:  # conv -> batchnorm -> rectify (m.res / the head convs)
     def __init__(self, w, gamma, beta):
         self.w, self.gamma, self.beta = w, gamma, beta
 
+    def conv(self, x):
+        return conv(x, self.w)
+
+    def batch_stats(self, z):
+        """per-channel mean and biased variance over (B, H, W)"""
+        return z.mean(axis=(0, 2, 3), keepdims=True), z.var(axis=(0, 2, 3), keepdims=True)
+
     def fwd(self, x, train):
         self.x = x
-        z = conv(x, self.w)
+        z = self.conv(x)
         if train:
-            mu = z.mean(axis=(0, 2, 3), keepdims=True)
-            var = z.var(axis=(0, 2, 3), keepdims=True)  # biased
+            mu, var = self.batch_stats(z)
             self.sd = np.sqrt(var + EPS)
             self.xhat = (z - mu) / self.sd
             y = self.gamma * self.xhat + self.beta
@@ -76,19 +82,20 @@ class Unit:  # conv -> batchnorm -> rectify (m.res / the head convs)
         dxhat = dy * self.gamma
         m1 = dxhat.mean(axis=(0, 2, 3), keepdims=True)
         m2 = (dxhat * self.xhat).mean(axis=(0, 2, 3), keepdims=True)
-        dz = (dxhat - m1 - self.xhat * m2) / self.sd
+        self.dz = dz = (dxhat - m1 - self.xhat * m2) / self.sd
         self.dw, dx = conv_bwd(self.x, self.w, dz)
         return dx
 
 
 class Net:
-    def __init__(self, tensors, shared_layers):
+    def __init__(self, tensors, shared_layers, unit=Unit):
+        """unit: the class of every conv unit (a subclass may override conv / batch_stats)"""
         t = [a for _, a in tensors]
         self.L = shared_layers
-        self.units = [Unit(*t[3 * i:3 * i + 3]) for i in range(1 + 2 * shared_layers)]
+        self.units = [unit(*t[3 * i:3 * i + 3]) for i in range(1 + 2 * shared_layers)]
         o = 3 * (1 + 2 * shared_layers)
-        self.pu = Unit(*t[o:o + 3]); self.pw, self.pb = t[o + 3], t[o + 4]
-        self.vu = Unit(*t[o + 5:o + 8]); self.vw, self.vb, self.ow, self.ob = t[o + 8], t[o + 9], t[o + 10], t[o + 11]
+        self.pu = unit(*t[o:o + 3]); self.pw, self.pb = t[o + 3], t[o + 4]
+        self.vu = unit(*t[o + 5:o + 8]); self.vw, self.vb, self.ow, self.ob = t[o + 8], t[o + 9], t[o + 10], t[o + 11]
 
     def forward(self, X, train):
         B = X.shape[0]

@@ -10,6 +10,9 @@ from agogo_b200 import _capi as K
 from tests import helpers as H
 from tests import pyref_dual as D
 
+# one training step of the fp32 oracle against float64: every tensor (every batch row of a batch-shaped one) within
+# TOL_GRAD of its own largest gradient, the cost within TOL_COST relative.  Measured at most 1.4e-6 and 6.2e-7.
+TOL_GRAD, TOL_COST = 6e-6, 2.5e-6
 
 @pytest.mark.parametrize("kind,m,n,k,nn", [
     (K.GAME_MNK, 3, 3, 3, dict(k=3, shared_layers=3, fc=8, batch_size=6, features=2, action_space=10)),
@@ -28,10 +31,19 @@ def test_dual_forward_and_gradients_vs_numpy(oracle, kind, m, n, k, nn):
     V = rng.choice([-1.0, 0.0, 1.0], B)
     go, co = e.train_grads(1, X.astype(np.float32).reshape(B, -1), Pi.astype(np.float32), V.astype(np.float32))
     cost, grads = net.loss_grads(X, Pi, V)
-    gp = D.pack(e, grads)
-    assert abs(co - cost) <= 1e-5 * max(1.0, abs(cost)), (co, cost)
-    scale = np.abs(gp).max()
-    assert np.abs(go - gp).max() <= 2e-4 * scale, (np.abs(go - gp).max(), scale)
+    assert abs(co - cost) <= TOL_COST * abs(cost), (co, cost)
+    # every tensor on its own scale, the batch-shaped ones (BatchNorm scale / bias, the linear biases) per batch row
+    worst = []
+    for i, g in enumerate(grads):
+        name, shape, off, size = e.param_desc(i)
+        d = np.abs(go[off:off + size].reshape(g.shape) - g)
+        rows = B if shape[0] == B and (name.endswith(("_γ", "_β")) or name.endswith("_b")) else 1
+        dm, gm = d.reshape(rows, -1).max(1), np.abs(g).reshape(rows, -1).max(1)
+        # a row whose reference is all zero (every unit of the sample rectified away) must be exactly zero
+        r = np.where(gm > 0, dm / np.where(gm > 0, gm, 1.0), np.where(dm > 0, np.inf, 0.0))
+        worst.append((float(r.max()), name))
+    print("worst per-tensor gradient ratio %.3g (%s), cost %.3g" % (*max(worst), abs(co - cost) / abs(cost)))
+    assert max(worst)[0] <= TOL_GRAD, sorted(worst)[-3:]
     # ---- inference (test-mode BatchNorm needs gains that keep 316x per layer finite: tame to ~1)
     H.tame_gammas([e], 0, 19, target=0.9)
     e.set_inferer(0, K.INF_DUAL)
