@@ -9,6 +9,8 @@
 // running the epilogue straight from its registers while the producer already fills the next tile's stages.
 // The number of tensor passes is a template parameter: a K block is one wgmma group with nothing between its wgmmas,
 // so ptxas emits one warpgroup.arrive per block instead of fencing every wgmma.
+// The fused layers' 192-row form (k_conv3x3_m192) runs the same body with three consumer warpgroups and no producer
+// warp: lane 0 of warp 0 issues the loads between its own K blocks.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -30,14 +32,20 @@ constexpr int NTHREADS = 288;  // warps 0-7: two consumer warpgroups; warp 8: TM
 constexpr int PRODUCER_WARP = 8;
 constexpr int CONSUMER_WARPS = 8;
 constexpr int TC_PASSES = 3;   // hi*hi + hi*lo + lo*hi (fp32-faithful); 2 drops lo*hi, 1 is hi*hi only (diagnostics)
+// k_conv3x3_m192: three consumer warpgroups x 64 rows, no producer warp (conv3x3_body)
+constexpr int BM192 = 192;
+constexpr int M192_THREADS = 384;
 // H100: 227 KB of dynamic shared memory per block, less alignment slack and the barriers
 constexpr int SMEM_RING_BUDGET = 227 * 1024 - 2048;
-// OPS: fp16 planes stored per operand — 2 = hi/lo (fp32-faithful), 1 = one fp16 (AZ_FLAG_FP16_TOWER)
-__host__ __device__ constexpr int stage_bytes(int BN, int OPS = 2) { return OPS * (BM * BK * 2 + BN * BK * 2); }
-__host__ __device__ constexpr int num_stages(int BN, int OPS = 2) {
-  return SMEM_RING_BUDGET / stage_bytes(BN, OPS) > 8 ? 8 : SMEM_RING_BUDGET / stage_bytes(BN, OPS);
+// OPS: fp16 planes stored per operand — 2 = hi/lo (fp32-faithful), 1 = one fp16 (AZ_FLAG_FP16_TOWER); bm: the M tile
+__host__ __device__ constexpr int stage_bytes(int BN, int OPS = 2, int bm = BM) { return OPS * (bm * BK * 2 + BN * BK * 2); }
+__host__ __device__ constexpr int num_stages(int BN, int OPS = 2, int bm = BM) {
+  return SMEM_RING_BUDGET / stage_bytes(BN, OPS, bm) > 8 ? 8 : SMEM_RING_BUDGET / stage_bytes(BN, OPS, bm);
 }
-__host__ __device__ constexpr int smem_bytes(int BN, int OPS = 2) { return num_stages(BN, OPS) * stage_bytes(BN, OPS) + 1024 + 256; }
+__host__ __device__ constexpr int smem_bytes(int BN, int OPS = 2, int bm = BM) {
+  return num_stages(BN, OPS, bm) * stage_bytes(BN, OPS, bm) + 1024 + 256;
+}
+static_assert(num_stages(256, 2, BM192) == 2, "the 192-row fused tile double-buffers its 112 KB stages");
 
 // The stored fp16 planes of an operand, and the tensor maps over them: hi and lo for the fp32-faithful form, hi alone for
 // the fp16 form, so that a kernel instantiated for one plane has no lo to read or write.
@@ -117,10 +125,19 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// im2col: consecutive pixels from (w, h, n) in W, H, N order over the map's bounding box, each read at (+dw, +dh);
+// positions off the tensor read as zeros
+__device__ __forceinline__ void tma_load_im2col(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c, int w, int h, int n,
+                                                uint16_t dw, uint16_t dh) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], "
+      "{%7, %8};"
+      ::"r"(dst), "l"(map), "r"(bar), "r"(c), "r"(w), "r"(h), "r"(n), "h"(dw), "h"(dh)
+      : "memory");
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// keeps the compiler from moving accumulator reads/writes across the asynchronous MMAs
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }// keeps the compiler from moving accumulator reads/writes across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
@@ -247,7 +264,7 @@ struct ConvArgs {
   int n_max;
   int S, Wp, H, W;    // positions per sample (flat: (H+1)*(W+1), per-sample: H*(W+1)), row pitch W+1
   int guard;          // zero rows in front of the activation buffers (flat layout only)
-  int mode3d, tps;    // per-sample layout: 3-D tensor map, tps = M tiles per sample
+  int mode3d, tps;    // per-sample layout: 3-D tensor map, tps = M tiles per sample of the launching kernel's tile
   int cin;            // padded input channels (multiple of 64)
   int n_total;        // GEMM N of the layer (fused: 2*K)
   int cout;           // output channels (K)
@@ -303,67 +320,101 @@ __device__ __forceinline__ float fused_value(const float2* aff, const float (&ac
 }
 
 // M tiles of a convolution over n samples: whole tiles per sample in the per-sample layout, else over the flat rows
-__host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n) {
-  return a.mode3d ? n * a.tps : (n * a.S + BM - 1) / BM;
+__host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n, int bm = BM) {
+  return a.mode3d ? n * a.tps : (n * a.S + bm - 1) / bm;
 }
 
+// The implicit-GEMM 3x3 convolution with WGS consumer warpgroups: an M tile of 64 * WGS rows.
+//   WGS = 2 (288 threads): warp 8 is the TMA producer (lane 0 issues the loads).
+//   WGS = 3 (384 threads): no producer warp.  A fourth warp would cap every thread at 152 registers (65536 / 416), and
+//   one m64n256k16 wgmma with its 128 fp32 accumulators needs more; ptxas allocates the whole kernel under the launch
+//   bound, so setmaxnreg cannot lend the consumers a producer warpgroup's registers either.  Lane 0 of warp 0 issues
+//   the loads instead: STAGES steps ahead before the first K block, then step it + STAGES as soon as its own warp has
+//   released step it.  It waits on the same empty barrier a producer warp would, so the loads start no later.
 // OPS = 2: activations and filters as fp16 hi/lo planes (out: hi/lo, or raw fp32 for training).  OPS = 1: one fp16
 // plane each, one pass (PASSES = 1), the output rounded once to fp16; half the bytes per stage, so a deeper ring.
 // Stage layout: A planes, then B planes.
-template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
-__global__ void __launch_bounds__(NTHREADS, 1)
-k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__ PlaneMaps<OPS> tmB, ConvArgs a,
-             Planes<OPS> out) {
+template <int WGS, int BN, bool PAIR, int PASSES, int OPS>
+__device__ __forceinline__ void conv3x3_body(const PlaneMaps<OPS>& tmA, const PlaneMaps<OPS>& tmB, const ConvArgs& a,
+                                             const Planes<OPS>& out) {
   static_assert(OPS == 2 || PASSES == 1, "a single fp16 plane has one pass");
-  constexpr int A_TILE_BYTES = BM * BK * 2;
-  constexpr int STAGES = num_stages(BN, OPS);
-  constexpr int STAGE_BYTES = stage_bytes(BN, OPS);
+  static_assert(WGS == 2 || WGS == 3, "two or three consumer warpgroups");
+  constexpr int TM = 64 * WGS;              // M tile
+  constexpr int CONSUMERS = 4 * WGS;        // consumer warps (WGS = 2: the producer warp is the next one)
+  constexpr int A_TILE_BYTES = TM * BK * 2;
+  constexpr int STAGES = num_stages(BN, OPS, TM);
+  constexpr int STAGE_BYTES = stage_bytes(BN, OPS, TM);
   constexpr int B_TILE_BYTES = BN * BK * 2;
   constexpr int OUTC = PAIR ? BN / 2 : BN;  // output channels per N tile
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const MbarRing<STAGES> ring{smem_base + STAGES * STAGE_BYTES};
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  ring.init(CONSUMER_WARPS);
+  ring.init(CONSUMERS);
   __syncthreads();
 
   const int n = min(*a.n_dev, a.n_max);
   const int rows = n * a.S;
-  const int m_tiles = conv_m_tiles(a, n);
+  // WGS = 3 on the per-sample layout: M runs over the n * H * W board points alone (im2col map, see below)
+  const int m_tiles = WGS == 3 && a.mode3d ? (n * a.H * a.W + TM - 1) / TM : conv_m_tiles(a, n, TM);
   const int n_tiles = a.n_total / BN;
   const int total_tiles = m_tiles * n_tiles;
   const int kc_per_tap = a.cin / BK;
   const int kblocks = 9 * kc_per_tap;
 
-  if (warp == PRODUCER_WARP) {
-    if (lane == 0) {
-      // ===== TMA producer =====
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-        const int m0 = mt * BM, n0 = nt * BN;
-        for (int kb = 0; kb < kblocks; kb++, it++) {
-          ring.producer_acquire(it, STAGE_BYTES);
-          const int tap = kb / kc_per_tap, kc = kb - tap * kc_per_tap;
-          const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-          const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES, bar = ring.full(it);
-          if (a.mode3d) {
-            const int b = mt / a.tps, p0 = (mt - b * a.tps) * BM + dy * a.Wp + dx;  // may be <0 / >=S: zero fill
-            tma_load_3d(sa, &tmA.hi, bar, kc * BK, p0, b);
-            if constexpr (OPS == 2) tma_load_3d(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, p0, b);
-          } else {
-            const int arow = a.guard + m0 + dy * a.Wp + dx;
-            tma_load_2d(sa, &tmA.hi, bar, kc * BK, arow);
-            if constexpr (OPS == 2) tma_load_2d(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, arow);
-          }
-          tma_load_2d(sa + OPS * A_TILE_BYTES, &tmB.hi, bar, tap * a.cin + kc * BK, n0);
-          if constexpr (OPS == 2) tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB.lo, bar, tap * a.cin + kc * BK, n0);
+  // pipeline step `it`: wait until the stage is free, then TMA K block kb of M tile mt (first row m0), N tile from row n0
+  const auto load_step = [&](uint32_t it, int mt, int m0, int n0, int kb) {
+    ring.producer_acquire(it, STAGE_BYTES);
+    const int tap = kb / kc_per_tap, kc = kb - tap * kc_per_tap;
+    const int dy = tap / 3 - 1, dx = tap % 3 - 1;
+    const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES, bar = ring.full(it);
+    if (WGS == 3 && a.mode3d) {
+      // the tile's first board point (b, y, x); the map's pixels start at the window corner (x - 1, y - 1) and each
+      // reads (+dx + 1, +dy + 1): tap (dy, dx), zero off the board
+      const int HW = a.H * a.W, b = m0 / HW, q = m0 - b * HW, y = q / a.W, x = q - y * a.W;
+      tma_load_im2col(sa, &tmA.hi, bar, kc * BK, x - 1, y - 1, b, (uint16_t)(dx + 1), (uint16_t)(dy + 1));
+      if constexpr (OPS == 2)
+        tma_load_im2col(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, x - 1, y - 1, b, (uint16_t)(dx + 1), (uint16_t)(dy + 1));
+    } else if (a.mode3d) {
+      const int b = mt / a.tps, p0 = (mt - b * a.tps) * TM + dy * a.Wp + dx;  // may be <0 / >=S: zero fill
+      tma_load_3d(sa, &tmA.hi, bar, kc * BK, p0, b);
+      if constexpr (OPS == 2) tma_load_3d(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, p0, b);
+    } else {
+      const int arow = a.guard + m0 + dy * a.Wp + dx;
+      tma_load_2d(sa, &tmA.hi, bar, kc * BK, arow);
+      if constexpr (OPS == 2) tma_load_2d(sa + A_TILE_BYTES, &tmA.lo, bar, kc * BK, arow);
+    }
+    tma_load_2d(sa + OPS * A_TILE_BYTES, &tmB.hi, bar, tap * a.cin + kc * BK, n0);
+    if constexpr (OPS == 2) tma_load_2d(sa + 2 * A_TILE_BYTES + B_TILE_BYTES, &tmB.lo, bar, tap * a.cin + kc * BK, n0);
+  };
+  // WGS = 3: the loading lane's cursor over this CTA's (tile, K block) steps
+  int p_tile = blockIdx.x, p_kb = 0;
+  uint32_t p_it = 0;
+  const auto load_next = [&]() {
+    if (p_tile >= total_tiles) return;
+    const int mt = p_tile / n_tiles;
+    load_step(p_it++, mt, mt * TM, (p_tile - mt * n_tiles) * BN, p_kb);
+    if (++p_kb == kblocks) { p_kb = 0; p_tile += gridDim.x; }
+  };
+
+  if constexpr (WGS == 2) {
+    if (warp == CONSUMERS) {
+      if (lane == 0) {
+        // ===== TMA producer =====
+        uint32_t it = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+          const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
+          const int m0 = mt * TM, n0 = nt * BN;
+          for (int kb = 0; kb < kblocks; kb++, it++) load_step(it, mt, m0, n0, kb);
         }
       }
+      return;
     }
-    return;
+  } else {
+    if (threadIdx.x == 0)
+      for (int s = 0; s < STAGES; s++) load_next();
   }
-  // ===== consumer warpgroups 0 and 1: rows wg*64 .. wg*64+63 of the tile =====
+  // ===== consumer warpgroups 0 .. WGS-1: rows wg*64 .. wg*64+63 of the tile =====
   const int wg = warp >> 2;
   int row0, col0;
   acc_frag_origin(warp, lane, row0, col0);
@@ -371,7 +422,7 @@ k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__
   uint32_t it = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int mt = tile / n_tiles, nt = tile - mt * n_tiles;
-    const int m0 = mt * BM, n0 = nt * BN;
+    const int m0 = mt * TM, n0 = nt * BN;
     for (int kb = 0; kb < kblocks; kb++, it++) {
       ring.consumer_wait(it);
       const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES;
@@ -382,6 +433,8 @@ k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__
       else
         mma_kblock<BN, 0, 1>(acc, make_desc_sw(sa + wg * 64 * 128), 0, make_desc_sw(sa + A_TILE_BYTES), 0, 32 >> 4, kb == 0);
       ring.consumer_release(it);
+      if constexpr (WGS == 3)
+        if (threadIdx.x == 0) load_next();  // step it + STAGES, into the stage just released
     }
     // ===== epilogue from registers =====
     bool overflow = false;
@@ -390,9 +443,14 @@ k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__
       const int lr = row0 + 8 * h;
       int r, p;  // r = row in the activation buffer (without guard), p = position inside the sample
       bool inb;
-      if (a.mode3d) {
+      if (WGS == 3 && a.mode3d) {  // row m0 + lr is board point q of sample b
+        const int HW = a.H * a.W, pt = m0 + lr, b = pt / HW, q = pt - b * HW;
+        p = q / a.W * a.Wp + q % a.W;
+        r = b * a.S + p;
+        inb = b < n;
+      } else if (a.mode3d) {
         const int b = mt / a.tps;
-        p = (mt - b * a.tps) * BM + lr;
+        p = (mt - b * a.tps) * TM + lr;
         r = b * a.S + p;
         inb = p < a.S;
       } else {
@@ -432,6 +490,21 @@ k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__
     }
     if (overflow) atomicOr(a.err, ERR_ACT_OVERFLOW);
   }
+}
+
+// 128-row tiles: every tower and training shape
+template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
+__global__ void __launch_bounds__(NTHREADS, 1)
+k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__ PlaneMaps<OPS> tmB, ConvArgs a,
+             Planes<OPS> out) {
+  conv3x3_body<2, BN, PAIR, PASSES, OPS>(tmA, tmB, a, out);
+}
+// 192-row tiles for the fused layers (hi/lo planes): 7/9 of the 128-row tile's operand bytes per MAC.  The activation
+// maps have 192-row boxes, and a.tps counts 192-row tiles per sample.
+template <int BN, bool PAIR, int PASSES = TC_PASSES>
+__global__ void __launch_bounds__(M192_THREADS, 1)
+k_conv3x3_m192(const __grid_constant__ PlaneMaps<2> tmA, const __grid_constant__ PlaneMaps<2> tmB, ConvArgs a, Planes<2> out) {
+  conv3x3_body<3, BN, PAIR, PASSES, 2>(tmA, tmB, a, out);
 }
 
 // dynamic shared memory opt-in of one instantiation on the current device (the attribute is per function and per device)
@@ -486,6 +559,33 @@ CUtensorMap make_map3d(void* base, uint64_t n, uint64_t S, uint64_t cols) {
   CUresult r = get_encode()(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeTiled(3d) failed: " + std::to_string((int)r));
+  return m;
+}
+
+// per-sample layout seen as the board alone: 4-D fp16 tensor [n][H][W][cols] over the [n][H][W+1][cols] buffer (the zero
+// column is skipped by the row stride), im2col boxes of `pixels` board points x 64 cols for a 3x3 window with padding 1:
+// the bounding box runs from corner offset -1 to -1, so pixel (x, y) starts at window corner (x - 1, y - 1)
+typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                   const int*, const int*, cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave,
+                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+CUtensorMap make_map_im2col(void* base, uint64_t n, uint64_t H, uint64_t W, uint64_t cols, uint32_t pixels) {
+  static EncodeIm2colFn fn = nullptr;
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    CUDA_CHECK(cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &q));
+    if (!p || q != cudaDriverEntryPointSuccess) throw std::runtime_error("cuTensorMapEncodeIm2col not available");
+    fn = (EncodeIm2colFn)p;
+  }
+  CUtensorMap m;
+  cuuint64_t dims[4] = {cols, W, H, n};
+  cuuint64_t strides[3] = {cols * 2, (W + 1) * cols * 2, H * (W + 1) * cols * 2};
+  int lower[2] = {-1, -1}, upper[2] = {-1, -1};
+  cuuint32_t es[4] = {1, 1, 1, 1};
+  CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, lower, upper, (cuuint32_t)BK, pixels, es,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) throw std::runtime_error("cuTensorMapEncodeIm2col failed: " + std::to_string((int)r));
   return m;
 }
 

@@ -19,6 +19,9 @@
 //   * warp roles (tc_common.cuh): one TMA producer warp, two consumer warpgroups of 64 rows each;
 //     smem ring of K-blocks (full/empty mbarriers), persistent CTAs striding over (M-tile, N-tile),
 //     epilogue (BN-affine + ReLU + branch add -> fp16 hi/lo split -> global) from the accumulators.
+//     The fused layers of K >= 128 nets run 192-row tiles (k_conv3x3_m192, three consumer warpgroups):
+//     fewer operand bytes per MAC, the same MMA sequence per row; on the per-sample layout the tiles
+//     cover the board points alone (TMA im2col), so the zero column and the tile tail cost no MMAs.
 // Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" table of wgmma.
 #include "tc_common.cuh"
 
@@ -286,6 +289,7 @@ void tower_configure_device() {
   set_conv_attr<256, true, 1>(); set_conv_attr<256, true, 2>(); set_conv_attr<128, true, 1>(); set_conv_attr<128, true, 2>();
   set_conv_attr<256, true, 1, 1>(); set_conv_attr<128, true, 1, 1>(); set_conv_attr<256, false, 1, 1>();
   set_conv_attr<128, false, 1, 1>(); set_conv_attr<64, false, 1, 1>();
+  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_m192<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256, 2, BM192)));
   CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small(2)));
   CUDA_CHECK(cudaFuncSetAttribute(k_smallnet_fp16, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small(1)));
 }
@@ -302,9 +306,11 @@ struct Impl {
   int n_max, ea, guard, S, rows_alloc, num_sms, passes = TC_PASSES, mode3d = 0, tps = 1;
   bool fp16 = false;   // AZ_FLAG_FP16_TOWER: one fp16 plane per operand (no *_lo buffers or maps), one pass
   bool small = false;  // K = 64, (H+1)(W+1) <= 128: the whole tower of a sample in one kernel (k_net_small / k_smallnet_fp16)
+  bool m192 = false;   // the fused layers run k_conv3x3_m192 (192-row tiles)
   __half *xin_hi = nullptr, *xin_lo = nullptr;  // [(guard+rows+guard)][64]
   __half *x_hi[2] = {nullptr, nullptr}, *x_lo[2] = {nullptr, nullptr};  // [(guard+rows+guard)][K]
   CUtensorMap mIn_hi, mIn_lo, mX_hi[2], mX_lo[2];
+  CUtensorMap mX192_hi[2], mX192_lo[2];  // the same buffers with 192-row boxes (m192 only)
   std::vector<Layer> layers;
   // profiling
   bool profile = false;
@@ -336,9 +342,10 @@ void launch_fused(int passes, const PlaneMaps<2>& A, const PlaneMaps<2>& B, cons
   else if (passes == 2) launch_conv<BN, true, 2>(A, B, a, out, num_sms, st);
   else launch_conv<BN, true>(A, B, a, out, num_sms, st);
 }
+// A192: the input's 192-row maps when the fused layers run k_conv3x3_m192 (I.m192), else nullptr
 template <int OPS>
-void dispatch_conv(const Impl& I, const Layer& L, const PlaneMaps<OPS>& A, const Planes<OPS>& out, const int* n_dev, int* err,
-                   cudaStream_t st) {
+void dispatch_conv(const Impl& I, const Layer& L, const PlaneMaps<OPS>& A, const PlaneMaps<OPS>* A192, const Planes<OPS>& out,
+                   const int* n_dev, int* err, cudaStream_t st) {
   ConvArgs a;
   a.n_dev = n_dev; a.n_max = I.n_max; a.S = I.S; a.Wp = I.d.W + 1; a.H = I.d.H; a.W = I.d.W; a.guard = I.guard;
   a.mode3d = I.mode3d; a.tps = I.tps;
@@ -346,6 +353,14 @@ void dispatch_conv(const Impl& I, const Layer& L, const PlaneMaps<OPS>& A, const
   a.act_scale = ldexpf(1.0f, I.ea); a.err = err;
   a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
   const PlaneMaps<OPS> B = maps_of<OPS>(L.mB_hi, L.mB_lo);
+  if constexpr (OPS == 2) {
+    if (A192 && L.pair && L.bn == 256) {
+      const int m_tiles = a.mode3d ? (a.n_max * a.H * a.W + BM192 - 1) / BM192 : conv_m_tiles(a, a.n_max, BM192);
+      const int grid = std::min(I.num_sms, m_tiles * (a.n_total / 256));
+      k_conv3x3_m192<256, true><<<grid, M192_THREADS, smem_bytes(256, 2, BM192), st>>>(*A192, B, a, out); LAUNCH_CHECK();
+      return;
+    }
+  }
   if constexpr (OPS == 1) {  // one pass whatever AZ_TC_PASSES says
     if (L.pair && L.bn == 256) launch_conv<256, true, 1, 1>(A, B, a, out, I.num_sms, st);
     else if (L.pair && L.bn == 128) launch_conv<128, true, 1, 1>(A, B, a, out, I.num_sms, st);
@@ -396,6 +411,19 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
     act_buf(d.K, I->x_hi[i], I->mX_hi[i]);
     if (!fp16) act_buf(d.K, I->x_lo[i], I->mX_lo[i]);
   }
+  // 192-row tiles for the fused layers (BN = 256: K >= 128) of the three-pass hi/lo tower.  On the per-sample layout
+  // their rows are the n * H * W board points alone, gathered by im2col maps (19x19: 361 rows per sample against 384 of
+  // the 128-row tiles); on the flat layout they are the flat rows, padded at the batch end only.  The storage layout
+  // above stays the 128-row one; TMA zero-fills what a box reads past it or off the board.
+  I->m192 = !fp16 && I->passes == TC_PASSES && d.K >= 128;
+  if (const char* m = getenv("AZ_TC_M192")) { if (m[0] == '0') I->m192 = false; }  // A/B: the 128-row kernel
+  if (I->m192)
+    for (int i = 0; i < 2; i++) {
+      __half* p[2] = {I->x_hi[i], I->x_lo[i]};
+      CUtensorMap* m[2] = {&I->mX192_hi[i], &I->mX192_lo[i]};
+      for (int j = 0; j < 2; j++)
+        *m[j] = I->mode3d ? make_map_im2col(p[j], n_max, d.H, d.W, d.K, BM192) : make_map(p[j], I->rows_alloc, d.K, BM192);
+    }
   // layers: init (single), then SharedLayers fused pairs
   const int K = d.K, HW = d.HW();
   for (int l = 0; l <= d.SharedLayers; l++) {
@@ -420,7 +448,7 @@ int tc_tower_kernel_kind(const TcTower& t) {
   const Impl* I = (const Impl*)t.impl;
   if (!I) return -1;
   if (I->fp16) return I->small ? 7 : 6;
-  return I->small ? 5 : 0;
+  return I->small ? 5 : I->m192 ? 8 : 0;
 }
 
 void tc_tower_free(TcTower& t) {
@@ -517,12 +545,13 @@ void tower_forward(Impl* I, const NetLayout& NL, const Snapshot& s, Fp32Scratch&
                                                                        scale, planes_of<OPS>(I->xin_hi, I->xin_lo)); LAUNCH_CHECK();
     if (launches) (*launches)++;
   }
-  dispatch_conv<OPS>(*I, I->layers[0], maps_of<OPS>(I->mIn_hi, I->mIn_lo), planes_of<OPS>(I->x_hi[0], I->x_lo[0]), n_dev, err_flag,
-                     st);
+  dispatch_conv<OPS>(*I, I->layers[0], maps_of<OPS>(I->mIn_hi, I->mIn_lo), nullptr, planes_of<OPS>(I->x_hi[0], I->x_lo[0]), n_dev,
+                     err_flag, st);
   if (launches) (*launches)++;
   for (size_t l = 1; l < I->layers.size(); l++) {
     size_t e0 = I->profile ? I->ev_get(st) : 0;
-    dispatch_conv<OPS>(*I, I->layers[l], maps_of<OPS>(I->mX_hi[cur], I->mX_lo[cur]),
+    const PlaneMaps<OPS> A192 = maps_of<OPS>(I->mX192_hi[cur], I->mX192_lo[cur]);
+    dispatch_conv<OPS>(*I, I->layers[l], maps_of<OPS>(I->mX_hi[cur], I->mX_lo[cur]), I->m192 ? &A192 : nullptr,
                        planes_of<OPS>(I->x_hi[cur ^ 1], I->x_lo[cur ^ 1]), n_dev, err_flag, st);
     if (I->profile) I->conv_spans.push_back({e0, I->ev_get(st)});
     if (launches) (*launches)++;

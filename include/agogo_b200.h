@@ -287,7 +287,8 @@ int az_counters_reset(az_engine* e);
  * forward_ms_total, forward_calls, region_ms, kernel_kind, 0...} accumulated since the last enable=1; region_ms is the
  * device time between the enable=1 and the enable=0 call on the engine's stream; kernel_kind names the kernel that runs
  * the fused layers (0 k_conv3x3_tc, wgmma, three fp16 passes; 5 k_net_small; 6 k_conv3x3_tc per layer in fp16, one pass
- * (AZ_FLAG_FP16_TOWER); 7 the fp16 small-net kernel k_smallnet_fp16; -1 fp32 tower; 1-4 were B200 kernels and are not used).  enable=2 times the region only (region_ms): no per-launch events, so
+ * (AZ_FLAG_FP16_TOWER); 7 the fp16 small-net kernel k_smallnet_fp16; 8 k_conv3x3_m192, the three-pass kernel on 192-row
+ * tiles (K >= 128; AZ_TC_M192=0 selects kind 0 instead); -1 fp32 tower; 1-4 were B200 kernels and are not used).  enable=2 times the region only (region_ms): no per-launch events, so
  * the captured wave graph keeps running — what a launch-bound small-net workload should be timed with. */
 int az_profile(az_engine* e, int32_t enable, double out[8]);
 
