@@ -7,8 +7,8 @@
 // stages (full/empty mbarriers); warps 0-7 are two consumer warpgroups, each owning 64 of the tile's 128 M rows and
 // issuing wgmma.mma_async (m64 x BN x k16, both operands from shared memory, fp32 accumulators in registers), then
 // running the epilogue straight from its registers while the producer already fills the next tile's stages.
-// The number of tensor passes is a template parameter: a K block is one wgmma group with nothing between its wgmmas,
-// so ptxas emits one warpgroup.arrive per block instead of fencing every wgmma.
+// The number of tensor passes follows from the operand form at compile time (mma_kblock): a K block is one wgmma group
+// with nothing between its wgmmas, so ptxas emits one warpgroup.arrive per block instead of fencing every wgmma.
 // The fused layers' 192-row form (k_conv3x3_m192) runs the same body with three consumer warpgroups and no producer
 // warp: lane 0 of warp 0 issues the loads between its own K blocks.
 #pragma once
@@ -31,7 +31,6 @@ constexpr int BK = 64;         // K block per pipeline stage: 64 fp16 = 128-byte
 constexpr int NTHREADS = 288;  // warps 0-7: two consumer warpgroups; warp 8: TMA producer
 constexpr int PRODUCER_WARP = 8;
 constexpr int CONSUMER_WARPS = 8;
-constexpr int TC_PASSES = 3;   // hi*hi + hi*lo + lo*hi (fp32-faithful); 2 drops lo*hi, 1 is hi*hi only (diagnostics)
 // k_conv3x3_m192: three consumer warpgroups x 64 rows, no producer warp (conv3x3_body)
 constexpr int BM192 = 192;
 constexpr int M192_THREADS = 384;
@@ -264,7 +263,7 @@ struct ConvArgs {
   int n_max;
   int S, Wp, H, W;    // positions per sample (flat: (H+1)*(W+1), per-sample: H*(W+1)), row pitch W+1
   int guard;          // zero rows in front of the activation buffers (flat layout only)
-  int mode3d, tps;    // per-sample layout: 3-D tensor map, tps = M tiles per sample of the launching kernel's tile
+  int mode3d, tps;    // per-sample layout: 3-D tensor map, tps = 128-row M tiles per sample
   int cin;            // padded input channels (multiple of 64)
   int n_total;        // GEMM N of the layer (fused: 2*K)
   int cout;           // output channels (K)
@@ -277,20 +276,23 @@ struct ConvArgs {
   const int* exp_b;
 };
 
-// One K block of the PASSES-pass product for this warpgroup's 64 rows: A rows at a_hi / a_lo, B (BN rows) at b_hi / b_lo.
+// One K block of the product for this warpgroup's 64 rows: A rows at a_hi / a_lo, B (BN rows) at b_hi / b_lo.  The
+// operand form sets the passes: OPS = 2 (hi/lo planes) runs hi*hi + hi*lo + lo*hi, fp32-faithful up to the dropped
+// lo*lo; OPS = 1 (one fp16 plane) runs hi*hi alone and leaves the lo descriptors unused.
 // a_step / b_step: descriptor start-address advance (16-byte units) per 16-wide K step.
-template <int BN, int TB, int PASSES = TC_PASSES>
+template <int BN, int TB, int OPS = 2>
 __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t dAh, uint64_t dAl, uint64_t dBh, uint64_t dBl,
                                            uint32_t b_step, bool first, uint32_t a_step = 32 >> 4) {
-  static_assert(PASSES >= 1 && PASSES <= 3, "1 to 3 passes");
   wgmma_fence();
 #pragma unroll
   for (int ks = 0; ks < BK / 16; ks++) {
     const uint64_t adv = (uint64_t)ks * a_step;     // A: K-major SWIZZLE_128B: 16 fp16 = 32 B inside the atom
     const uint64_t advb = (uint64_t)ks * b_step;    // B: K-major as A; MN-major 16 K-rows of 128 B
     wgmma_f16<BN, TB>(acc, dAh + adv, dBh + advb, (first && ks == 0) ? 0u : 1u);
-    if constexpr (PASSES >= 2) wgmma_f16<BN, TB>(acc, dAh + adv, dBl + advb, 1u);
-    if constexpr (PASSES >= 3) wgmma_f16<BN, TB>(acc, dAl + adv, dBh + advb, 1u);
+    if constexpr (OPS == 2) {
+      wgmma_f16<BN, TB>(acc, dAh + adv, dBl + advb, 1u);
+      wgmma_f16<BN, TB>(acc, dAl + adv, dBh + advb, 1u);
+    }
   }
   wgmma_commit();
   wgmma_wait_all();
@@ -319,9 +321,13 @@ __device__ __forceinline__ float fused_value(const float2* aff, const float (&ac
   return v * act_scale;
 }
 
-// M tiles of a convolution over n samples: whole tiles per sample in the per-sample layout, else over the flat rows
-__host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n, int bm = BM) {
-  return a.mode3d ? n * a.tps : (n * a.S + bm - 1) / bm;
+// M tiles of a convolution over n samples for the kernel with WGS consumer warpgroups (64 * WGS rows per tile).  Per-sample
+// layout: WGS = 3 tiles the n * H * W board points alone (im2col maps), WGS = 2 has whole 128-row tiles per sample.  Flat
+// layout: tiles over the flat rows.
+__host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n, int WGS) {
+  const int tm = 64 * WGS;
+  if (WGS == 3 && a.mode3d) return (n * a.H * a.W + tm - 1) / tm;
+  return a.mode3d ? n * a.tps : (n * a.S + tm - 1) / tm;
 }
 
 // The implicit-GEMM 3x3 convolution with WGS consumer warpgroups: an M tile of 64 * WGS rows.
@@ -332,12 +338,11 @@ __host__ __device__ __forceinline__ int conv_m_tiles(const ConvArgs& a, int n, i
 //   the loads instead: STAGES steps ahead before the first K block, then step it + STAGES as soon as its own warp has
 //   released step it.  It waits on the same empty barrier a producer warp would, so the loads start no later.
 // OPS = 2: activations and filters as fp16 hi/lo planes (out: hi/lo, or raw fp32 for training).  OPS = 1: one fp16
-// plane each, one pass (PASSES = 1), the output rounded once to fp16; half the bytes per stage, so a deeper ring.
+// plane each, one pass, the output rounded once to fp16; half the bytes per stage, so a deeper ring.
 // Stage layout: A planes, then B planes.
-template <int WGS, int BN, bool PAIR, int PASSES, int OPS>
+template <int WGS, int BN, bool PAIR, int OPS>
 __device__ __forceinline__ void conv3x3_body(const PlaneMaps<OPS>& tmA, const PlaneMaps<OPS>& tmB, const ConvArgs& a,
                                              const Planes<OPS>& out) {
-  static_assert(OPS == 2 || PASSES == 1, "a single fp16 plane has one pass");
   static_assert(WGS == 2 || WGS == 3, "two or three consumer warpgroups");
   constexpr int TM = 64 * WGS;              // M tile
   constexpr int CONSUMERS = 4 * WGS;        // consumer warps (WGS = 2: the producer warp is the next one)
@@ -355,8 +360,7 @@ __device__ __forceinline__ void conv3x3_body(const PlaneMaps<OPS>& tmA, const Pl
 
   const int n = min(*a.n_dev, a.n_max);
   const int rows = n * a.S;
-  // WGS = 3 on the per-sample layout: M runs over the n * H * W board points alone (im2col map, see below)
-  const int m_tiles = WGS == 3 && a.mode3d ? (n * a.H * a.W + TM - 1) / TM : conv_m_tiles(a, n, TM);
+  const int m_tiles = conv_m_tiles(a, n, WGS);
   const int n_tiles = a.n_total / BN;
   const int total_tiles = m_tiles * n_tiles;
   const int kc_per_tap = a.cin / BK;
@@ -426,12 +430,9 @@ __device__ __forceinline__ void conv3x3_body(const PlaneMaps<OPS>& tmA, const Pl
     for (int kb = 0; kb < kblocks; kb++, it++) {
       ring.consumer_wait(it);
       const uint32_t sa = smem_base + ring.stage(it) * STAGE_BYTES;
-      if constexpr (OPS == 2)
-        mma_kblock<BN, 0, PASSES>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
-                                  make_desc_sw(sa + 2 * A_TILE_BYTES), make_desc_sw(sa + 2 * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
-                                  kb == 0);
-      else
-        mma_kblock<BN, 0, 1>(acc, make_desc_sw(sa + wg * 64 * 128), 0, make_desc_sw(sa + A_TILE_BYTES), 0, 32 >> 4, kb == 0);
+      mma_kblock<BN, 0, OPS>(acc, make_desc_sw(sa + wg * 64 * 128), make_desc_sw(sa + A_TILE_BYTES + wg * 64 * 128),
+                             make_desc_sw(sa + OPS * A_TILE_BYTES), make_desc_sw(sa + OPS * A_TILE_BYTES + B_TILE_BYTES), 32 >> 4,
+                             kb == 0);
       ring.consumer_release(it);
       if constexpr (WGS == 3)
         if (threadIdx.x == 0) load_next();  // step it + STAGES, into the stage just released
@@ -493,32 +494,42 @@ __device__ __forceinline__ void conv3x3_body(const PlaneMaps<OPS>& tmA, const Pl
 }
 
 // 128-row tiles: every tower and training shape
-template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
+template <int BN, bool PAIR, int OPS = 2>
 __global__ void __launch_bounds__(NTHREADS, 1)
 k_conv3x3_tc(const __grid_constant__ PlaneMaps<OPS> tmA, const __grid_constant__ PlaneMaps<OPS> tmB, ConvArgs a,
              Planes<OPS> out) {
-  conv3x3_body<2, BN, PAIR, PASSES, OPS>(tmA, tmB, a, out);
+  conv3x3_body<2, BN, PAIR, OPS>(tmA, tmB, a, out);
 }
 // 192-row tiles for the fused layers (hi/lo planes): 7/9 of the 128-row tile's operand bytes per MAC.  The activation
-// maps have 192-row boxes, and a.tps counts 192-row tiles per sample.
-template <int BN, bool PAIR, int PASSES = TC_PASSES>
+// maps have 192-row boxes.
+template <int BN, bool PAIR>
 __global__ void __launch_bounds__(M192_THREADS, 1)
 k_conv3x3_m192(const __grid_constant__ PlaneMaps<2> tmA, const __grid_constant__ PlaneMaps<2> tmB, ConvArgs a, Planes<2> out) {
-  conv3x3_body<3, BN, PAIR, PASSES, 2>(tmA, tmB, a, out);
+  conv3x3_body<3, BN, PAIR, 2>(tmA, tmB, a, out);
 }
 
+// The conv kernel with WGS consumer warpgroups, its block size and its dynamic shared memory
+template <int WGS, int BN, bool PAIR, int OPS>
+constexpr auto conv_kernel() {
+  if constexpr (WGS == 2) return k_conv3x3_tc<BN, PAIR, OPS>;
+  else return k_conv3x3_m192<BN, PAIR>;
+}
+constexpr int conv_threads(int WGS) { return WGS == 2 ? NTHREADS : M192_THREADS; }
+constexpr int conv_smem_bytes(int WGS, int BN, int OPS) { return smem_bytes(BN, OPS, 64 * WGS); }
+
 // dynamic shared memory opt-in of one instantiation on the current device (the attribute is per function and per device)
-template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
+template <int WGS, int BN, bool PAIR, int OPS = 2>
 void set_conv_attr() {
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_tc<BN, PAIR, PASSES, OPS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  smem_bytes(BN, OPS)));
+  CUDA_CHECK(cudaFuncSetAttribute(conv_kernel<WGS, BN, PAIR, OPS>(), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  conv_smem_bytes(WGS, BN, OPS)));
 }
 // persistent grid: one CTA per SM, or one per tile when the largest batch has fewer
-template <int BN, bool PAIR, int PASSES = TC_PASSES, int OPS = 2>
+template <int WGS, int BN, bool PAIR, int OPS = 2>
 void launch_conv(const PlaneMaps<OPS>& A, const PlaneMaps<OPS>& B, const ConvArgs& a, const Planes<OPS>& out, int num_sms,
                  cudaStream_t st) {
-  const int grid = std::min(num_sms, conv_m_tiles(a, a.n_max) * (a.n_total / BN));
-  k_conv3x3_tc<BN, PAIR, PASSES, OPS><<<grid, NTHREADS, smem_bytes(BN, OPS), st>>>(A, B, a, out); LAUNCH_CHECK();
+  const int grid = std::min(num_sms, conv_m_tiles(a, a.n_max, WGS) * (a.n_total / BN));
+  const auto kernel = conv_kernel<WGS, BN, PAIR, OPS>();
+  kernel<<<grid, conv_threads(WGS), conv_smem_bytes(WGS, BN, OPS), st>>>(A, B, a, out); LAUNCH_CHECK();
 }
 
 // ---------------------------------------------------------------------------------------------

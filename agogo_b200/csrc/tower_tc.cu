@@ -19,7 +19,7 @@
 //   * warp roles (tc_common.cuh): one TMA producer warp, two consumer warpgroups of 64 rows each;
 //     smem ring of K-blocks (full/empty mbarriers), persistent CTAs striding over (M-tile, N-tile),
 //     epilogue (BN-affine + ReLU + branch add -> fp16 hi/lo split -> global) from the accumulators.
-//     The fused layers of K >= 128 nets run 192-row tiles (k_conv3x3_m192, three consumer warpgroups):
+//     The fused layers of K >= 128 nets on hi/lo planes run 192-row tiles (k_conv3x3_m192, three consumer warpgroups):
 //     fewer operand bytes per MAC, the same MMA sequence per row; on the per-sample layout the tiles
 //     cover the board points alone (TMA im2col), so the zero column and the tile tail cost no MMAs.
 // Descriptor bit layouts follow the PTX ISA "Matrix Descriptor Format" table of wgmma.
@@ -170,12 +170,8 @@ __device__ __forceinline__ void small_layer(const SmallNetArgs<OPS>& a, int l, i
     ring.consumer_wait(it);
     const uint32_t shift = (uint32_t)(SN_R0 + wg * 64 + (tap / 3 - 1) * a.Wp + (tap % 3 - 1)) * 16;
     const uint32_t sb = stages + ring.stage(it) * sn_stage_bytes(OPS);
-    if constexpr (OPS == 2)
-      mma_kblock<N, 0>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_hi + SN_PLANE + shift, SN_HR * 16),
-                       make_desc_sw(sb), make_desc_sw(sb + SN_TILE), 32 >> 4, tap == 0, 2 * SN_HR * 16 >> 4);
-    else
-      mma_kblock<N, 0, 1>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), 0, make_desc_sw(sb), 0, 32 >> 4, tap == 0,
-                          2 * SN_HR * 16 >> 4);
+    mma_kblock<N, 0, OPS>(acc, make_desc_plain(in_hi + shift, SN_HR * 16), make_desc_plain(in_hi + SN_PLANE + shift, SN_HR * 16),
+                          make_desc_sw(sb), make_desc_sw(sb + SN_TILE), 32 >> 4, tap == 0, 2 * SN_HR * 16 >> 4);
     ring.consumer_release(it);
   }
   const bool last = l == a.nlayers - 1;
@@ -284,12 +280,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_smallnet_fp16(const __grid_cons
 // dynamic shared memory opt-in of every instantiation this file launches, on the current device (called from the
 // allocator, which runs with the engine's device current)
 void tower_configure_device() {
-  set_conv_attr<256, true>(); set_conv_attr<128, true>(); set_conv_attr<256, false>(); set_conv_attr<128, false>();
-  set_conv_attr<64, false>();
-  set_conv_attr<256, true, 1>(); set_conv_attr<256, true, 2>(); set_conv_attr<128, true, 1>(); set_conv_attr<128, true, 2>();
-  set_conv_attr<256, true, 1, 1>(); set_conv_attr<128, true, 1, 1>(); set_conv_attr<256, false, 1, 1>();
-  set_conv_attr<128, false, 1, 1>(); set_conv_attr<64, false, 1, 1>();
-  CUDA_CHECK(cudaFuncSetAttribute(k_conv3x3_m192<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256, 2, BM192)));
+  set_conv_attr<3, 256, true>();
+  set_conv_attr<2, 256, true>(); set_conv_attr<2, 128, true>(); set_conv_attr<2, 256, false>(); set_conv_attr<2, 128, false>();
+  set_conv_attr<2, 64, false>();
+  set_conv_attr<2, 256, true, 1>(); set_conv_attr<2, 128, true, 1>(); set_conv_attr<2, 256, false, 1>();
+  set_conv_attr<2, 128, false, 1>(); set_conv_attr<2, 64, false, 1>();
   CUDA_CHECK(cudaFuncSetAttribute(k_net_small, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small(2)));
   CUDA_CHECK(cudaFuncSetAttribute(k_smallnet_fp16, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes_small(1)));
 }
@@ -303,7 +298,7 @@ struct Layer {
 };
 struct Impl {
   NetDims d;
-  int n_max, ea, guard, S, rows_alloc, num_sms, passes = TC_PASSES, mode3d = 0, tps = 1;
+  int n_max, ea, guard, S, rows_alloc, num_sms, mode3d = 0, tps = 1;
   bool fp16 = false;   // AZ_FLAG_FP16_TOWER: one fp16 plane per operand (no *_lo buffers or maps), one pass
   bool small = false;  // K = 64, (H+1)(W+1) <= 128: the whole tower of a sample in one kernel (k_net_small / k_smallnet_fp16)
   bool m192 = false;   // the fused layers run k_conv3x3_m192 (192-row tiles)
@@ -334,14 +329,6 @@ template <int OPS> PlaneMaps<OPS> maps_of(const CUtensorMap& hi, const CUtensorM
   else return {hi};
 }
 
-// AZ_TC_PASSES (diagnostics) selects 1 or 2 passes for the fused layers; the other shapes always run three
-template <int BN>
-void launch_fused(int passes, const PlaneMaps<2>& A, const PlaneMaps<2>& B, const ConvArgs& a, const Planes<2>& out, int num_sms,
-                  cudaStream_t st) {
-  if (passes == 1) launch_conv<BN, true, 1>(A, B, a, out, num_sms, st);
-  else if (passes == 2) launch_conv<BN, true, 2>(A, B, a, out, num_sms, st);
-  else launch_conv<BN, true>(A, B, a, out, num_sms, st);
-}
 // A192: the input's 192-row maps when the fused layers run k_conv3x3_m192 (I.m192), else nullptr
 template <int OPS>
 void dispatch_conv(const Impl& I, const Layer& L, const PlaneMaps<OPS>& A, const PlaneMaps<OPS>* A192, const Planes<OPS>& out,
@@ -353,29 +340,14 @@ void dispatch_conv(const Impl& I, const Layer& L, const PlaneMaps<OPS>& A, const
   a.act_scale = ldexpf(1.0f, I.ea); a.err = err;
   a.out_raw = nullptr; a.exp_a = nullptr; a.exp_b = nullptr;
   const PlaneMaps<OPS> B = maps_of<OPS>(L.mB_hi, L.mB_lo);
-  if constexpr (OPS == 2) {
-    if (A192 && L.pair && L.bn == 256) {
-      const int m_tiles = a.mode3d ? (a.n_max * a.H * a.W + BM192 - 1) / BM192 : conv_m_tiles(a, a.n_max, BM192);
-      const int grid = std::min(I.num_sms, m_tiles * (a.n_total / 256));
-      k_conv3x3_m192<256, true><<<grid, M192_THREADS, smem_bytes(256, 2, BM192), st>>>(*A192, B, a, out); LAUNCH_CHECK();
-      return;
-    }
-  }
-  if constexpr (OPS == 1) {  // one pass whatever AZ_TC_PASSES says
-    if (L.pair && L.bn == 256) launch_conv<256, true, 1, 1>(A, B, a, out, I.num_sms, st);
-    else if (L.pair && L.bn == 128) launch_conv<128, true, 1, 1>(A, B, a, out, I.num_sms, st);
-    else if (!L.pair && L.bn == 256) launch_conv<256, false, 1, 1>(A, B, a, out, I.num_sms, st);
-    else if (!L.pair && L.bn == 128) launch_conv<128, false, 1, 1>(A, B, a, out, I.num_sms, st);
-    else if (!L.pair && L.bn == 64) launch_conv<64, false, 1, 1>(A, B, a, out, I.num_sms, st);
-    else throw std::runtime_error("tc tower: unsupported tile");
-  } else {
-    if (L.pair && L.bn == 256) launch_fused<256>(I.passes, A, B, a, out, I.num_sms, st);
-    else if (L.pair && L.bn == 128) launch_fused<128>(I.passes, A, B, a, out, I.num_sms, st);
-    else if (!L.pair && L.bn == 256) launch_conv<256, false>(A, B, a, out, I.num_sms, st);
-    else if (!L.pair && L.bn == 128) launch_conv<128, false>(A, B, a, out, I.num_sms, st);
-    else if (!L.pair && L.bn == 64) launch_conv<64, false>(A, B, a, out, I.num_sms, st);
-    else throw std::runtime_error("tc tower: unsupported tile");
-  }
+  if constexpr (OPS == 2)  // the 192-row kernel exists for hi/lo planes only
+    if (A192 && L.pair && L.bn == 256) return launch_conv<3, 256, true>(*A192, B, a, out, I.num_sms, st);
+  if (L.pair && L.bn == 256) launch_conv<2, 256, true, OPS>(A, B, a, out, I.num_sms, st);
+  else if (L.pair && L.bn == 128) launch_conv<2, 128, true, OPS>(A, B, a, out, I.num_sms, st);
+  else if (!L.pair && L.bn == 256) launch_conv<2, 256, false, OPS>(A, B, a, out, I.num_sms, st);
+  else if (!L.pair && L.bn == 128) launch_conv<2, 128, false, OPS>(A, B, a, out, I.num_sms, st);
+  else if (!L.pair && L.bn == 64) launch_conv<2, 64, false, OPS>(A, B, a, out, I.num_sms, st);
+  else throw std::runtime_error("tc tower: unsupported tile");
 }
 
 }  // namespace
@@ -390,7 +362,6 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
   Impl* I = new Impl;
   t.impl = I;
   I->d = d; I->n_max = n_max; I->ea = act_scale_log2; I->fp16 = fp16;
-  if (const char* ps = getenv("AZ_TC_PASSES")) { int v = atoi(ps); if (v >= 1 && v <= 3) I->passes = v; }  // experiments only
   // layout choice by padded-row overhead (rows computed per real board point)
   const int S_flat = (d.H + 1) * (d.W + 1), S_ps = d.H * (d.W + 1), tps = (S_ps + BM - 1) / BM;
   I->mode3d = (tps * BM < S_flat) ? 1 : 0;
@@ -415,7 +386,7 @@ void tc_tower_alloc(TcTower& t, const NetDims& d, int n_max, int act_scale_log2,
   // their rows are the n * H * W board points alone, gathered by im2col maps (19x19: 361 rows per sample against 384 of
   // the 128-row tiles); on the flat layout they are the flat rows, padded at the batch end only.  The storage layout
   // above stays the 128-row one; TMA zero-fills what a box reads past it or off the board.
-  I->m192 = !fp16 && I->passes == TC_PASSES && d.K >= 128;
+  I->m192 = !fp16 && d.K >= 128;
   if (const char* m = getenv("AZ_TC_M192")) { if (m[0] == '0') I->m192 = false; }  // A/B: the 128-row kernel
   if (I->m192)
     for (int i = 0; i < 2; i++) {

@@ -201,7 +201,7 @@ __global__ void k_prep_filter(const float* __restrict__ w, int Co, int Ci, int c
 
 // dynamic shared memory opt-in of the instantiations this file launches (per function, per device)
 void train_configure_device() {
-  set_conv_attr<256, false>(); set_conv_attr<128, false>(); set_conv_attr<64, false>();
+  set_conv_attr<2, 256, false>(); set_conv_attr<2, 128, false>(); set_conv_attr<2, 64, false>();
   CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(256)));
   CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(128)));
   CUDA_CHECK(cudaFuncSetAttribute(k_dw_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes(64)));
@@ -326,9 +326,9 @@ void tc_gemm_conv(TcGemm& g, const float* x, int Cin, const float* filter, int f
   a.cin = cpad; a.n_total = Cout; a.cout = Cout; a.aff = nullptr; a.act_scale = 1.0f;
   a.err = nullptr; a.out_raw = I->raw; a.exp_a = sl.exp; a.exp_b = I->exp_b;
   const Planes<2> none{nullptr, nullptr};  // raw mode: the epilogue writes out_raw
-  if (bn == 256) launch_conv<256, false>(mA, mB, a, none, I->num_sms, st);
-  else if (bn == 128) launch_conv<128, false>(mA, mB, a, none, I->num_sms, st);
-  else launch_conv<64, false>(mA, mB, a, none, I->num_sms, st);
+  if (bn == 256) launch_conv<2, 256, false>(mA, mB, a, none, I->num_sms, st);
+  else if (bn == 128) launch_conv<2, 128, false>(mA, mB, a, none, I->num_sms, st);
+  else launch_conv<2, 64, false>(mA, mB, a, none, I->num_sms, st);
   k_unpack_nchw<<<dim3((HW + 31) / 32, (Cout + 31) / 32, I->B), 256, 0, st>>>(I->raw, I->B, Cout, d.H, d.W, Cout, I->guard, I->S, out, accumulate ? 1 : 0); LAUNCH_CHECK();
   if (launches) *launches += nl + 4;
 }

@@ -40,8 +40,8 @@ USEFUL_POLICY_REL, USEFUL_VALUE = 5e-2, 1e-2
 # position
 C3_TOL = {"tamed": (9e-4, 1.8e-4), "reference": (2.3e-2, 4e-3)}
 
-# the fp16 kernels: k_conv3x3_tc<BN, PAIR, PASSES = 1, OPS = 1> for the five tower shapes, and the fp16 small net
-FP16_CONV = ["k_conv3x3_tcILi%dELb%dELi1ELi1EE" % s for s in ((256, 1), (128, 1), (256, 0), (128, 0), (64, 0))]
+# the fp16 kernels: k_conv3x3_tc<BN, PAIR, OPS = 1> for the five tower shapes, and the fp16 small net
+FP16_CONV = ["k_conv3x3_tcILi%dELb%dELi1EE" % s for s in ((256, 1), (128, 1), (256, 0), (128, 0), (64, 0))]
 FP16_SMALL = "k_smallnet_fp16"
 
 

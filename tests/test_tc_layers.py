@@ -31,8 +31,10 @@ DEFAULT_ACT_SCALE_LOG2 = -2  # what act_scale_log2 = 0 selects
 # |dev - ref| / (2^-21 * (mag + |ref| + 2^-(4 + act_scale_log2))) over every layer and element of a case is the last
 # column of TOWER_CASES; 1.68 at K = 64, 2.32 at K = 128, 2.97 at K = 256, so the bound leaves about 4x.
 C_TOWER = 6.5
-# AZ_TC_PASSES=2 drops the lo(x) * hi(w) pass, so the activations enter as fp16 (2^-12 relative): measured 128 to 172 on
-# the fused layers of wq13-k64, 20x to 26x the bound.  The test asks for 16x.
+# Dropping the lo(x) * hi(w) pass makes the activations enter as fp16 (2^-12 relative).  On the fused layers of wq13-k64
+# the former two-pass diagnostic build measured 128 to 172 on an H100 SXM (80 GB, 700 W), 20x to 26x the bound; the
+# float64 restatement of that product in test_bound_catches_a_dropped_pass gives 124 to 173, 19x to 27x.  The test asks
+# for 16x.
 PASSES2_MIN_EXCESS = 16.0
 # heads: relative error of every policy entry, absolute error of the value (measured at most 5.2e-7 and 2.1e-7)
 TOL_POLICY, TOL_VALUE = 2e-6, 1e-6
@@ -239,17 +241,43 @@ def test_tower_layers_vs_float64(engine_lib, monkeypatch, c):
     assert rel_p.max() <= TOL_POLICY and dv.max() <= TOL_VALUE, (c.name, rel_p.max(), dv.max())
 
 
-@pytest.mark.gpu
-def test_bound_catches_a_dropped_pass(engine_lib, monkeypatch):
-    """The per-layer bound is tight enough to see a real precision loss: AZ_TC_PASSES=2 (diagnostics) drops the
-    lo(x) * hi(w) pass of the fused layers, and their worst ratio must exceed the bound many times over.  A layered case:
-    k_net_small ignores the variable, and the init conv always runs three passes."""
+def _split_hi_lo(v):
+    """The device's operand split of v rounded to fp32: hi = fp16(v), lo = fp16(v - hi), both returned in float64."""
+    v = np.asarray(v, np.float32)
+    hi = v.astype(np.float16)
+    lo = (v - hi.astype(np.float32)).astype(np.float16)
+    return hi.astype(np.float64), lo.astype(np.float64)
+
+
+def test_bound_catches_a_dropped_pass(oracle):
+    """The per-layer bound is tight enough to see a real precision loss: the fused layers of wq13-k64 without the
+    lo(x) * hi(w) pass, restated in float64, must exceed it many times over.  Each layer's input is stored as the device
+    stores it (x * 2^act_scale_log2 as fp16 hi + lo), its filters are taken at their per-layer power-of-two scale and
+    split the same way (tc_tower_prepare), and hi(x) * (hi(w) + lo(w)) goes through the layer's affine, ReLU and branch
+    add; the reference is the exact layer on the same stored input."""
     c = next(c for c in TOWER_CASES if c.name == "wq13-k64")
-    worst, *_, deep = _tower_layers(engine_lib, monkeypatch, c, env={"AZ_TC_PASSES": "2"})
-    deep.close()
-    print("AZ_TC_PASSES=2 %s: worst ratio per layer %s" % (c.name, " ".join("%.3g" % w for w in worst)))
-    assert worst[0] <= c_tower(c.k)
-    assert min(worst[1:]) >= PASSES2_MIN_EXCESS * c_tower(c.k), worst
+    e = oracle.create(_desc(c.kind, c.m, c.n, c.k, c.layers, c.n_big))
+    H.tame_gammas([e], 0, 11, target=0.9)
+    net = D.Net(D.unpack(e, 0), c.layers)
+    e.close()
+    x = _planes(c.kind, np.random.default_rng(11), c.n_big, c.m, c.n).reshape(c.n_big, -1, c.m, c.n).astype(np.float64)
+    x = _layer_ref(net, 0, x)[0]
+    scale = 2.0 ** DEFAULT_ACT_SCALE_LOG2
+    worst = []
+    for l in range(1, c.layers + 1):
+        x_hi, x_lo = _split_hi_lo(x * scale)
+        ref, mag = _layer_ref(net, l, (x_hi + x_lo) / scale)
+        units = [net.units[2 * l - 1], net.units[2 * l]]
+        ew = 7 - int(np.frexp(max(np.abs(u.w).max() for u in units))[1])  # max |w| * 2^ew in [64, 128)
+        out = 0.0
+        for u in units:
+            w_hi, w_lo = _split_hi_lo(np.ldexp(u.w, ew))
+            z = D.conv(x_hi / scale, np.ldexp(w_hi + w_lo, -ew))
+            out = out + np.maximum(u.gamma[0] / np.sqrt(D.EPS) * z + u.beta[0], 0)
+        worst.append(float(_ratio(out, ref, mag, 0).max()))
+        x = ref
+    print("%s without lo(x) * hi(w): worst ratio per fused layer %s" % (c.name, " ".join("%.3g" % w for w in worst)))
+    assert min(worst) >= PASSES2_MIN_EXCESS * c_tower(c.k), worst
 
 
 @pytest.mark.gpu

@@ -18,7 +18,7 @@ from tests import pyref_dual as D
 from tests.test_tc_layers import _desc, _planes, tower_layout
 from tests.test_tower_pipeline import K_STEPS_PER_BLOCK, LIB, TC_PASSES, _cuobjdump, _sass_functions
 
-M192 = "k_conv3x3_m192ILi256ELb1ELi3EE"
+M192 = "k_conv3x3_m192ILi256ELb1EE"
 BM192 = 192
 MAX_REGS = 168  # 384 threads x 168 = 64512 of the SM's 65536 registers, one CTA per SM
 
