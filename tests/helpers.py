@@ -117,6 +117,23 @@ def play_and_collect(e, n_games, record=True, dump_trees=True, max_plies=10000):
     return dict(dumps=dumps, records=recs, examples=ex, stats=stats, states=states, counters=e.counters())
 
 
+def tree_children(rows):
+    """Parent row of every row of a preorder tree dump (-1 for the root) and the children rows of every row, in list
+    order: the children of row i are the next rows at depth + 1 until the depth drops back."""
+    depth = rows[:, 0]
+    parent = np.full(len(rows), -1, np.int64)
+    kids = {}
+    stack = []
+    for i, d in enumerate(depth):
+        while stack and depth[stack[-1]] >= d:
+            stack.pop()
+        if stack:
+            parent[i] = stack[-1]
+            kids.setdefault(stack[-1], []).append(i)
+        stack.append(i)
+    return parent, kids
+
+
 def assert_same_run(a, b, what="", float_ulps=0):
     """float_ulps=0: every tree field bit-identical.  float_ulps>0 (network-in-the-loop runs only):
     structure, moves and visit counts identical, W and P within that many fp32 ulps — the engine's

@@ -554,19 +554,11 @@ def test_graph_replay_equals_plain_launches(engine_lib):
 
 def _check_tree_invariants(rows, sims_done_total):
     """Size-independent properties of a search tree dump (rows: depth, move, N, Wbits, Pbits, expanded, nchild)."""
-    depth, N, nchild, expanded = rows[:, 0], rows[:, 2].astype(np.int64), rows[:, 6], rows[:, 5]
+    N, nchild, expanded = rows[:, 2].astype(np.int64), rows[:, 6], rows[:, 5]
     P = rows[:, 4].copy().view(np.float32)
     W = rows[:, 3].copy().view(np.float32)
     assert np.isfinite(W).all() and np.isfinite(P).all()
-    # walk the preorder dump: children of row i are the next rows at depth+1 until depth drops back
-    stack = []
-    kids = {}
-    for i, d in enumerate(depth):
-        while stack and depth[stack[-1]] >= d:
-            stack.pop()
-        if stack:
-            kids.setdefault(stack[-1], []).append(i)
-        stack.append(i)
+    _, kids = H.tree_children(rows)
     for i in range(len(rows)):
         ch = kids.get(i, [])
         assert len(ch) == nchild[i]
